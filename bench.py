@@ -1,14 +1,15 @@
 #!/usr/bin/env python
-"""bench.py -- SDF points/sec of the DISN hot path (BASELINE.json metric: 256^3 grid, 1/2/4/8 x B200).
+"""bench.py -- SDF points/sec of the DISN hot path (BASELINE.json metric: 256^3 grid, 1/2/4/8 x H100).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 0|1|2|4] [--precision P]
+                    [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic 137x137 images: encode (resize + VGG-16 + the folds)
 then the dense (res+1)^3 SDF grid per image (projection + multi-scale gather + two-stream MLP + /10).
 
     --config 1 (default; with --gpus N > 1 it is BASELINE config 3): single image, --sdf_res 256 (257^3 points).
     --config 0: single image, --sdf_res 64 (the reference's own CPU-runnable case, 2 chunks of 137 313 points).
-    --config 2: batch of 8 images, --sdf_res 128 (8 x 129^3 points), VGG on tcgen05; adds the encoder's images/s.
+    --config 2: batch of 8 images, --sdf_res 128 (8 x 129^3 points), VGG on the tensor cores; adds the encoder's images/s.
     --config 4: single image, --sdf_res 512 (513^3 points) + CUDA marching-cubes post-pass on rank 0 inside the step.
 
 With N GPUs the grid's z-slabs are sharded across ranks (strong scaling: total work fixed), every rank re-encodes the
@@ -20,6 +21,10 @@ epilogue; `--gather nccl` uses an NCCL gather instead), inside the timed region.
            caller-pinned buffers: the image crosses PCIe inside the step and the kernel's epilogue stores the SDF straight
            into the pinned host grid (no device staging, no trailing copy).  With N > 1 every rank writes its slab into one
            shared pinned host grid (POSIX shared memory registered with cudaHostRegister), each over its own PCIe link.
+`--dump-outputs DIR`: after the timed steps, writes what the last timed step computed -- the SDF grid -- as
+           DIR/sdf_plane_mid.npy (the middle z-plane of every image, [B, R, R]) and DIR/sdf_sample.npy (a fixed, seeded sample of
+           2^21 grid values, flat indices in DIR/sdf_sample_index.npy), float32 / float64, so that two builds can be compared
+           output for output on identical inputs.
 `--impl reference`: the CPU oracle restating the reference's TF graph (TF itself is not installable here), all host
            threads, reference loop structure (whole graph incl. VGG per chunk).  Each step is a bounded sample of the SAME
            workload: one full chunk as the reference executes it (config 0: the whole 2-chunk job).
@@ -59,7 +64,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(bf16_burst=d["bf16_tflops"], bf16_sustained=d["bf16_tflops_sustained"], hbm=d["hbm_gbs"],
                     source="measured")
-    return dict(bf16_burst=1590.0, bf16_sustained=1400.0, hbm=6650.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3; 700 W part): upper bounds, not reached rates
+    return dict(bf16_burst=989.0, bf16_sustained=989.0, hbm=3350.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -232,6 +238,21 @@ def shared_pinned_grid(nfloats: int, rank: int, world: int, barrier):
     return t, cleanup
 
 
+DUMP_SAMPLES = 1 << 21
+
+
+def dump_outputs(out_dir: str, grid: np.ndarray):
+    """The SDF grid of the last timed step: every image's middle z-plane plus a fixed, seeded sample of all values
+    (at most 2^21 x 12 bytes + B x R^2 x 4 bytes, under 64 MB for every config)."""
+    os.makedirs(out_dir, exist_ok=True)
+    flat = grid.reshape(-1)
+    idx = np.random.default_rng(20240601).choice(flat.size, size=min(DUMP_SAMPLES, flat.size), replace=False)
+    idx.sort()
+    np.save(os.path.join(out_dir, "sdf_plane_mid.npy"), np.ascontiguousarray(grid[:, grid.shape[1] // 2], dtype=np.float32))
+    np.save(os.path.join(out_dir, "sdf_sample.npy"), flat[idx].astype(np.float32))
+    np.save(os.path.join(out_dir, "sdf_sample_index.npy"), idx.astype(np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -340,6 +361,13 @@ def run_ours(args):
         else:
             eng.eval_grid(sp, tm_np, res, out=host_np)
 
+    def full_grid():        # rank 0: the [B, R, R, R] result of the last step, on the host
+        if world == 1:
+            return slab.cpu().numpy()
+        if peer:
+            return eng.fetch(shared_ptr, (B, R, R, R))
+        return torch.cat([g[:, :z_bounds[r + 1] - z_bounds[r]].cpu() for r, g in enumerate(gathered)], 1).numpy()
+
     def timed(fn, steps):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -376,6 +404,8 @@ def run_ours(args):
     clocks = sampler.stop() if rank == 0 else None
     ms_step = ms_total / args.steps
     value = total_pts / (ms_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, full_grid())
 
     # kernel-only duration of the dominant kernel (fused point kernel) on this rank's slab, and of the encoder
     def ev_time(fn, reps):
@@ -423,24 +453,13 @@ def run_ours(args):
     # the host grid now holds the e2e result: cross-check it against the device-resident one
     e2e_ok = None
     if rank == 0 and B == 1 and not do_mc:
-        if world == 1:
-            dev_grid = slab.cpu()
-        elif peer:
-            dev_grid = torch.from_numpy(eng.fetch(shared_ptr, (B, R, R, R)))
-        else:
-            dev_grid = torch.cat([g[:, :z_bounds[r + 1] - z_bounds[r]].cpu() for r, g in enumerate(gathered)], 1)
+        dev_grid = torch.from_numpy(full_grid())
         e2e_ok = bool(torch.equal(host_grid.view(B, R, R, R), dev_grid))
 
     if rank == 0:
         peaks = load_peaks()
         achieved = slab_pts * F_ALG / (k_ms * 1e-3) / 1e12
         peak = peaks["bf16_sustained"]
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "point_kernel_traffic.json")
-        if os.path.exists(tpath) and world == 1:
-            t = json.load(open(tpath)).get(args.precision)
-            if t and t.get("sdf_res") == res and B == 1:
-                traffic = t["dram_bytes_read"] + t["dram_bytes_write"]
         passes = {"bf16x3": 3.0, "f16f8": 58.0 / 33.0}.get(args.precision, 1.0)     # bf16-rate MMA units per product (f16f8: 1.5 in fold2/conv1, 2 elsewhere)
         dtype_s = {"fp32": "f32",
                    "bf16x3": "bf16x3 (bf16 hi/lo split operands, 3 MMAs/product, fp32 accumulate)",
@@ -457,15 +476,15 @@ def run_ours(args):
                        if world > 1 else "z-slab x1",
                        "l2": "inputs larger than L2: each step streams 554 MB of VGG weights + writes %.0f MB of SDF" % (total_pts * 4 / 1e6)},
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                         "frac": achieved / peak, "traffic": traffic, "kernel": "fused point kernel (%s)" % args.precision,
+                         "frac": achieved / peak, "kernel": "fused point kernel (%s)" % args.precision,
                          "kernel_ms": k_ms, "flop_per_point": F_ALG,
                          "algorithmic_bytes": int(slab_pts * 4),
                          "executed_tflops": achieved * passes,
                          "note": "frac counts the algorithmic FLOPs once; the split-operand scheme spends %.2fx that in bf16-rate tensor-pipe time"
                                  % passes if passes > 1 else "CUDA-core fp32 path reported against the tensor roofline",
-                         "peak_source": "%s bf16 sustained (MEASURED_PEAKS.json)" % peaks["source"]},
+                         "peak_source": "%s bf16" % peaks["source"]},
             "encoder": {"ms": enc_ms, "images_per_s": B / (enc_ms * 1e-3), "batch": B,
-                        "note": "resize + VGG-16 (tcgen05 convs) + fc6-8 + global/local folds, CUDA-graph replay"},
+                        "note": "resize + VGG-16 (tensor-core convs) + fc6-8 + global/local folds, CUDA-graph replay"},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(img_host.numel() * 4 + tm_host.numel() * 4),
                     "d2h_bytes_per_step": int(total_pts * 4) if not do_mc else int((mesh.get("nv", 0) + mesh.get("nf", 0)) * 12),
                     "ms_per_step": ms_e2e,
@@ -513,6 +532,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--clock-period-ms", type=int, default=100, dest="clock_period_ms",
                     help="nvidia-smi sampling period during the timed region (0 = one sample right after it)")
+    ap.add_argument("--dump-outputs", default=None, dest="dump_outputs", metavar="DIR",
+                    help="write the last timed step's SDF grid (middle planes + a seeded sample) as .npy files to DIR")
     ap.add_argument("--gather", default="peer", choices=["peer", "nccl"],
                     help="N > 1: how the z-slabs reach rank 0's HBM (peer = stores from the kernel epilogue over NVLink)")
     args = ap.parse_args()

@@ -1,7 +1,7 @@
 """ctypes binding of libdisn_b200.so (the C ABI declared in include/disn_b200.h).
 
 There is no CPU or eager fallback: if the shared library is missing it is built with nvcc, and if that
-fails -- or no sm_100 GPU is present when a context is created -- the error is raised to the caller.
+fails -- or no sm_90 GPU is present when a context is created -- the error is raised to the caller.
 """
 from __future__ import annotations
 

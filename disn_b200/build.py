@@ -1,4 +1,4 @@
-"""Build libdisn_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libdisn_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -15,7 +15,7 @@ SOURCES = ["api.cu", "encoder.cu", "point_fp32.cu", "point_tc.cu", "mc.cu", "cha
 DIAG_SOURCES = ["tc_selftest.cu", "tc_probe.cu"]
 EXTRA_FLAGS = {"iou.cu": ["--fmad=false"]}     # voxel classification must match the float64 oracle operation for operation
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC,-ffp-contract=off", "--expt-relaxed-constexpr", "-shared"]
 
 

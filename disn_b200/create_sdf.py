@@ -1,7 +1,7 @@
 """Drop-in mirror of the reference's inference driver ``test/create_sdf.py`` (and ``demo/demo.py``) for the
 SDF hot path: same module-level constants, same function names and argument meaning
 (``create``, ``test_one_epoch``, ``to_binary``, ``create_obj``, ``create_one_cube_obj``), running on the
-B200 library.  Dataset loading (``TEST_DATASET``: h5 files on disk) is out of scope: ``create`` takes an
+DISN library.  Dataset loading (``TEST_DATASET``: h5 files on disk) is out of scope: ``create`` takes an
 iterable of ``batch_data`` dicts in the loader's layout (data/data_sdf_h5_queue.py:291-303).
 
     import disn_b200.create_sdf as cs

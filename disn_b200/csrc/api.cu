@@ -1,4 +1,4 @@
-// C ABI of the DISN B200 hot-path library (see include/disn_b200.h for the reference call sites).
+// C ABI of the DISN hot-path library (see include/disn_b200.h for the reference call sites).
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -37,15 +37,15 @@ int disn_create(const disn_config* cfg, disn_ctx** out) {
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev == 0) {
-    set_error(std::string("no CUDA device: the DISN B200 path has no CPU fallback (") + cudaGetErrorString(e) + ")");
+    set_error(std::string("no CUDA device: the DISN path has no CPU fallback (") + cudaGetErrorString(e) + ")");
     return -1;
   }
   DISN_REQUIRE(cfg->device >= 0 && cfg->device < ndev, "device ordinal out of range");
   DISN_CUDA_OK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   DISN_CUDA_OK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) {
-    set_error("this library is built for sm_100a (B200) only; device is sm_" + std::to_string(prop.major) +
+  if (prop.major != 9) {
+    set_error("this library is built for sm_90a (H100) only; device is sm_" + std::to_string(prop.major) +
               std::to_string(prop.minor));
     return -1;
   }
@@ -456,7 +456,7 @@ int disn_write_obj(const char* path, const float* verts, int64_t n_verts, const 
   if (!f) { set_error(std::string("cannot open ") + path); return -3; }
   std::vector<char> buf(1 << 20);
   setvbuf(f, buf.data(), _IOFBF, buf.size());
-  fprintf(f, "# Generated by the DISN B200 marching-cubes post-pass\n# Number of vertices: %lld\n# Number of faces: %lld\n",
+  fprintf(f, "# Generated by the DISN marching-cubes post-pass\n# Number of vertices: %lld\n# Number of faces: %lld\n",
           (long long)n_verts, (long long)n_faces);
   for (int64_t i = 0; i < n_verts; ++i) fprintf(f, "v %g %g %g\n", verts[3 * i], verts[3 * i + 1], verts[3 * i + 2]);
   for (int64_t i = 0; i < n_faces; ++i)

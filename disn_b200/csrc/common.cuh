@@ -1,4 +1,4 @@
-// Shared declarations for the DISN B200 library (sm_100a only).
+// Shared declarations for the DISN library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -97,7 +97,7 @@ struct disn_ctx {
   std::map<std::string, disn::DevTensor> weights;
   bool weights_dirty = true;
   int64_t launches = 0;
-  int num_sms = 148;            // cudaDevAttrMultiProcessorCount of cfg.device, read once in disn_create
+  int num_sms = 132;            // cudaDevAttrMultiProcessorCount of cfg.device, read once in disn_create
   bool attr_conv_tc = false, attr_point_fp32 = false;   // cudaFuncSetAttribute done on this device
   std::set<const void*> attr_done;                      // ... for the point_tc_kernel instantiations
 
@@ -129,7 +129,7 @@ struct disn_ctx {
   float* d_axes = nullptr;      // [max_batch,3,R]
   int32_t axes_R = 0;
   std::vector<double> axes_key; // (sdf_params, R) the tables in d_axes were built from
-  // bf16x3 packed weights (tcgen05 path)
+  // bf16x3 packed weights (tensor-core path)
   void* tc_weights = nullptr;          // bf16 hi/lo stage images of the point MLP (DISN_PREC_BF16X3)
   int64_t tc_weights_bytes = 0;
   void* tc_weights_f8 = nullptr;       // fp16 + e5m2 stage images (DISN_PREC_F16F8)

@@ -1,4 +1,4 @@
-// Image encoder of the DISN hot path, fp32 CUDA-core implementation for sm_100a.
+// Image encoder of the DISN hot path, fp32 CUDA-core implementation for sm_90a.
 //
 // Restates (not ports) models/model_normalization.py:65-77 (137->224 legacy bilinear resize, vgg_16 with
 // num_classes=1024, is_training=False) and the per-image part of :171-190 after two exact algebraic folds
@@ -223,9 +223,9 @@ static int launch_gemm(disn_ctx* c, int mode, const float* A, const float* Bm, c
   const int BN = (N % 128 == 0) ? 128 : 64;
   if (N % 64 != 0) { set_error("gemm: N must be a multiple of 64"); return -2; }
   const int ctas = (N / BN) * ((M + 127) / 128);
-  // split-K so that small late layers (few output tiles) still fill 148 SMs for ~2 waves
+  // split-K so that small late layers (few output tiles) still fill the SMs for ~2 waves
   int splits = 1;
-  if (K % 8 == 0 && ctas < 148) {
+  if (K % 8 == 0 && ctas < c->num_sms) {
     const int kchunks = K / 64 > 0 ? K / 64 : 1;             // keep >= 64 k per split
     int want = (296 + ctas - 1) / ctas;
     if (want > kchunks) want = kchunks;
@@ -241,7 +241,7 @@ static int launch_gemm(disn_ctx* c, int mode, const float* A, const float* Bm, c
   c->launches++;
   if (splits > 1) {
     const int64_t mn4 = (int64_t)M * N / 4;
-    int blocks = (int)std::min<int64_t>((mn4 + 255) / 256, 148 * 8);
+    int blocks = (int)std::min<int64_t>((mn4 + 255) / 256, c->num_sms * 8);
     splitk_reduce_kernel<<<blocks, 256, 0, c->stream>>>(reinterpret_cast<const float4*>(ws), bias,
                                                        reinterpret_cast<float4*>(C), mn4, N / 4, splits, relu);
     c->launches++;
@@ -250,7 +250,7 @@ static int launch_gemm(disn_ctx* c, int mode, const float* A, const float* Bm, c
   return 0;
 }
 
-// GEMM dispatcher: tcgen05 path (bf16 hi/lo split, fp32 accumulate) when the context runs in DISN_PREC_BF16X3 and
+// GEMM dispatcher: tensor-core path (bf16 hi/lo split, fp32 accumulate) when the context runs in DISN_PREC_BF16X3 and
 // the shapes fit (K % 64 == 0, channels % 64 == 0); fp32 CUDA-core path otherwise (conv1_1: Cin = 3).
 static int gemm_any(disn_ctx* c, const std::string& wname, int mode, const float* A, const float* Bm, const float* bias,
                     float* C, int M, int N, int K, int relu, ConvGeom g) {
@@ -265,7 +265,7 @@ static int gemm_any(disn_ctx* c, const std::string& wname, int mode, const float
     return -1;
   if (splits > 1) {
     const int64_t mn4 = (int64_t)M * N / 4;
-    int blocks = (int)std::min<int64_t>((mn4 + 255) / 256, 148 * 8);
+    int blocks = (int)std::min<int64_t>((mn4 + 255) / 256, c->num_sms * 8);
     splitk_reduce_kernel<<<blocks, 256, 0, c->stream>>>(reinterpret_cast<const float4*>(c->splitk_ws), bias,
                                                        reinterpret_cast<float4*>(C), mn4, N / 4, splits, relu);
     c->launches++;
@@ -454,7 +454,7 @@ int encoder_alloc(disn_ctx* c, int B) {
 }  // namespace disn
 #ifdef DISN_DIAGNOSTICS
 // Diagnostic: run one GEMM (plain if H == 0, else 3x3 SAME im2col of an NHWC tensor) through both the fp32
-// CUDA-core kernel and the tcgen05 kernel; host pointers.  Used by the GPU test-suite to sweep shapes.
+// CUDA-core kernel and the tensor-core kernel; host pointers.  Used by the GPU test-suite to sweep shapes.
 extern "C" int disn_debug_gemm(disn_ctx* c, const float* A, const float* Wt, const float* bias, int M, int N, int K,
                                int H, int Wd, int Cin, int relu, float* out_fp32, float* out_tc) {
   using namespace disn;
@@ -511,7 +511,7 @@ static int encoder_body(disn_ctx* c, int B, int H, int W, int C, bool embedding_
 
 // The encoder is ~50 small launches (13 convs with split-K reduces, pools, GEMVs, 5 projections, the map fold): at B = 1
 // their GPU time is ~0.5 ms but the launch gaps made it ~3 ms per step.  After one eager run per shape (which also packs
-// the tcgen05 weight images), the launch sequence is captured into a CUDA graph and replayed with one cudaGraphLaunch.
+// the tensor-core weight images), the launch sequence is captured into a CUDA graph and replayed with one cudaGraphLaunch.
 void encoder_graph_reset(disn_ctx* c) {
   if (c->enc_graph_exec) cudaGraphExecDestroy(c->enc_graph_exec);
   c->enc_graph_exec = nullptr;
@@ -603,7 +603,7 @@ static int encoder_body(disn_ctx* c, int B, int H, int W, int C, bool embedding_
     if (is_tap) {
       float* p = c->act[pp];
       int64_t total = (int64_t)B * (hw / 2) * (hw / 2) * (kConvCout[i] / 4);
-      int blocks = (int)std::min<int64_t>((total + 255) / 256, 148 * 8);
+      int blocks = (int)std::min<int64_t>((total + 255) / 256, c->num_sms * 8);
       maxpool2_kernel<<<blocks, 256, 0, c->stream>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(p),
                                                      B, hw, hw, kConvCout[i] / 4);
       c->launches++;
@@ -642,7 +642,7 @@ static int encoder_body(disn_ctx* c, int B, int H, int W, int C, bool embedding_
       float* tmp = c->act[0];
       const int oh = c->cfg.img_h;
       const int64_t total = (int64_t)B * oh * oh * kTapC[l];
-      resize_bilinear_tf_kernel<<<(int)std::min<int64_t>((total + 255) / 256, 148 * 16), 256, 0, c->stream>>>(
+      resize_bilinear_tf_kernel<<<(int)std::min<int64_t>((total + 255) / 256, c->num_sms * 16), 256, 0, c->stream>>>(
           c->taps[l], tmp, B, hw, hw, kTapC[l], oh, oh);
       c->launches++;
       src = tmp;
@@ -658,7 +658,7 @@ static int encoder_body(disn_ctx* c, int B, int H, int W, int C, bool embedding_
   }
   {
     int64_t total = (int64_t)B * c->cfg.img_h * c->cfg.img_w * (kHidden / 4);
-    int blocks = (int)std::min<int64_t>((total + 255) / 256, 148 * 16);
+    int blocks = (int)std::min<int64_t>((total + 255) / 256, c->num_sms * 16);
     pmap_accumulate_kernel<<<blocks, 256, 0, c->stream>>>(lv, reinterpret_cast<float4*>(c->pmap), B, c->cfg.img_h,
                                                           c->cfg.img_w);
     c->launches++;

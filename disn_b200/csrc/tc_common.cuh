@@ -1,5 +1,5 @@
-// sm_100a building blocks for the tensor-core point kernel: mbarrier, cluster, bulk-copy (TMA engine),
-// TMEM allocation, UMMA descriptors, tcgen05.mma (cta_group::2) and tcgen05.ld wrappers (inline PTX).
+// sm_90a building blocks for the tensor-core kernels: mbarrier, cluster, bulk copy (TMA engine), GMMA shared-memory
+// descriptors and warpgroup MMA (wgmma.mma_async, m64n128) wrappers (inline PTX).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -40,8 +40,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 // arrive on the barrier at the same smem offset in CTA `cta_rank` of the cluster
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta_rank) {
   uint32_t remote = mapa(smem_u32(bar), cta_rank);
-  // default semantics (.release at .cta scope), as CUTLASS's ClusterBarrier::arrive(cta_id): the signalled data is
-  // consumed by this CTA's own async proxy (tensor core reading this CTA's smem), already ordered by fence.proxy.async
   asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
@@ -49,18 +47,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// acquire at cluster scope: needed when the arrival came from the peer CTA's generic-proxy stores/arrives
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
       "selp.b32 %0, 1, 0, p;\n\t}"
       : "=r"(ok)
       : "r"(smem_u32(bar)), "r"(parity)
@@ -90,26 +76,13 @@ static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parit
   }
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;      // try_wait itself suspends for a HW time slice when not ready
+  if (mbar_try_wait(bar, parity)) return;
   mbar_wait_slow(bar, parity);
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  uint64_t t0 = 0;
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if ((++spins & 0xFFFu) == 0) {
-      const uint64_t now = globaltimer_ns();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > DISN_MBAR_TIMEOUT_NS) __trap();
-    }
-  }
 }
 
 // ---------------------------------------------------------------- proxies / fences -------------------
-// generic-proxy smem writes -> visible to the async proxy (UMMA operand reads, bulk copies)
+// generic-proxy smem writes -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ---------------------------------------------------------------- bulk copy (TMA engine, 1-D) --------
 // global -> this CTA's shared memory, completion counted in bytes on a local mbarrier
@@ -123,69 +96,6 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 // L1 prefetch of the 128-byte line holding `p` (generic address of global memory); a pure hint
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.L1 [%0];" ::"l"(p)); }
 
-// ---------------------------------------------------------------- TMEM -------------------------------
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_cg2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// 32 lanes x 32-bit x 32 consecutive columns: thread t of warp w gets lane 32*(w%4)+t
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- UMMA descriptors -------------------
-// K-major operand tile, 128-byte swizzle: rows of 64 bf16 (128 B), 8-row groups 1024 B apart, tile base
-// 1024-B aligned.  (cute::UMMA::SmemDescriptor: version=1, layout_type=SWIZZLE_128B, SBO=1024>>4, LBO=1.)
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// advance along K by `k_elems` bf16 inside the 64-wide swizzle atom (start address += bytes>>4)
-__device__ __forceinline__ uint64_t desc_advance_k(uint64_t desc, uint32_t k_elems) {
-  return desc + (uint64_t)((k_elems * 2u) >> 4);
-}
-// instruction descriptor: D=f32, A=B=bf16, both K-major, dense
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T, issued by ONE thread of the leader CTA for the CTA pair
-__device__ __forceinline__ void mma_cg2(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}"
-      :
-      : "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-// arrive (once) on the barrier at this smem offset in every CTA of `cta_mask` when all prior MMAs retire
-__device__ __forceinline__ void commit_cg2(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// --- warp-uniform issue path: the whole MMA warp runs the loop, one elected lane issues ----------------
-// (keeps descriptors/addresses in uniform registers instead of ELECT+R2UR per operand in divergent code)
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -195,52 +105,94 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-// high 32 bits of every K-major SW128 descriptor (SBO=64, version=1, layout_type=2); low word = addr>>4 | LBO
-constexpr uint32_t kDescHi = 64u | (1u << 14) | (2u << 29);
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr) { return ((smem_addr >> 4) & 0x3FFFu) | (1u << 16); }
-__device__ __forceinline__ void mma_cg2_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %3, {%6, %6, %6, %6, %6, %6, %6, %6}, p;\n\t}"
-      :
-      : "r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHi), "r"(0u)
-      : "memory");
-}
 
-// ---- mixed-kind path (DISN_PREC_F16F8): fp16 main product + e5m2 correction products in one accumulator ----
-// instruction descriptor with A=B=fp16 (kind::f16) -- formats 0; for kind::f8f6f4 format 1 = E5M2, i.e. the same bits as
-// make_idesc_bf16 (cute::UMMA::InstrDescriptor: a_format [7,10), b_format [10,13)).
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N) {
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t make_idesc_e5m2(uint32_t M, uint32_t N) { return make_idesc_bf16(M, N); }
-// K-major SWIZZLE_64B tile of 1-byte elements: rows of 64 B, 8-row groups 512 B apart (SBO=32), layout_type=4
-constexpr uint32_t kDescHiSw64 = 32u | (1u << 14) | (4u << 29);
-__host__ __device__ constexpr uint32_t sw64_offset(uint32_t row, uint32_t chunk) {
-  return (row >> 3) * 512u + (row & 7u) * 64u + ((chunk ^ ((row >> 1) & 3u)) << 4);
-}
-// kind::f8f6f4, K = 32 per instruction, both operands SW64 tiles
-__device__ __forceinline__ void mma_cg2_f8_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], da, db, %3, {%6, %6, %6, %6, %6, %6, %6, %6}, p;\n\t}"
-      :
-      : "r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw64), "r"(0u)
-      : "memory");
-}
-
-// swizzled byte offset of 16-byte chunk `chunk` (0..7) of row `row` in a K-major SW128 tile
+// ---------------------------------------------------------------- operand tiles ----------------------
+// K-major SWIZZLE_128B tile of 2-byte elements: rows of 64 elements (128 B), 8-row groups 1024 B apart, tile base
+// 1024-B aligned.  Byte offset of 16-byte chunk `chunk` (0..7) of row `row`:
 __host__ __device__ constexpr uint32_t sw128_offset(uint32_t row, uint32_t chunk) {
   return (row >> 3) * 1024u + (row & 7u) * 128u + ((chunk ^ (row & 7u)) << 4);
 }
+// K-major SWIZZLE_64B tile of 1-byte elements: rows of 64 B, 8-row groups 512 B apart
+__host__ __device__ constexpr uint32_t sw64_offset(uint32_t row, uint32_t chunk) {
+  return (row >> 3) * 512u + (row & 7u) * 64u + ((chunk ^ ((row >> 1) & 3u)) << 4);
+}
+
+// GMMA shared-memory matrix descriptor (sm_90): start address >> 4 in [0,14), leading byte offset >> 4 in [16,30)
+// (unused for swizzled K-major tiles, 1), stride byte offset >> 4 in [32,46) (one 8-row group), swizzle mode in
+// [62,64) (1 = 128 B, 2 = 64 B).  Moving along K inside the swizzle atom adds bytes >> 4 to the start address.
+constexpr uint32_t kDescHiSw128 = 64u | (1u << 30);
+constexpr uint32_t kDescHiSw64 = 32u | (2u << 30);
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t smem_addr) {
+  return ((uint64_t)kDescHiSw128 << 32) | (uint64_t)(((smem_addr >> 4) & 0x3FFFu) | (1u << 16));
+}
+__device__ __forceinline__ uint64_t desc_sw64(uint32_t smem_addr) {
+  return ((uint64_t)kDescHiSw64 << 32) | (uint64_t)(((smem_addr >> 4) & 0x3FFFu) | (1u << 16));
+}
+
+// ---------------------------------------------------------------- warpgroup MMA ----------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait points
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// operand kinds of wgmma_m64n128: 2-byte kinds take K = 16 per instruction, e5m2 takes K = 32
+enum { KIND_BF16 = 0, KIND_F16 = 1, KIND_E5M2 = 2 };
+
+#define DISN_WGMMA_D64                                                                                                \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "   \
+  "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define DISN_WGMMA_OPS64                                                                                             \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),       \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),         \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),        \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),        \
+      "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),        \
+      "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),        \
+      "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),        \
+      "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+
+// D[64 x 128] (+)= A[64 x K] * B[128 x K]^T, both operands K-major in shared memory, fp32 accumulators in registers.
+// Fragment of thread t of the warpgroup (warp w = t/32, lane l): d[4j + e] = D[16w + l/4 + 8(e/2)][8j + 2(l%4) + e%2].
+template <int kKind>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (kKind == KIND_BF16) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " DISN_WGMMA_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : DISN_WGMMA_OPS64
+                 : "l"(da), "l"(db), "r"(accumulate));
+  } else if constexpr (kKind == KIND_F16) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " DISN_WGMMA_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : DISN_WGMMA_OPS64
+                 : "l"(da), "l"(db), "r"(accumulate));
+  } else {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k32.f32.e5m2.e5m2 " DISN_WGMMA_D64 ", %64, %65, p, 1, 1;\n\t}"
+                 : DISN_WGMMA_OPS64
+                 : "l"(da), "l"(db), "r"(accumulate));
+  }
+}
+
+// D[64 x 64] (+)= A[64 x 32] * B[64 x 32]^T in e5m2 (both K-major SW64 tiles); fragment as wgmma_m64n128, j < 8
+__device__ __forceinline__ void wgmma_m64n64_e5m2(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k32.f32.e5m2.e5m2 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void acc_fence(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#undef DISN_WGMMA_D64
+#undef DISN_WGMMA_OPS64
 
 // split fp32 pair into packed bf16 hi and packed bf16 lo (x ~= hi + lo, |x - hi - lo| <= 2^-17 |x|)
 __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
@@ -251,34 +203,4 @@ __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uin
   lo = *reinterpret_cast<uint32_t*>(&l);
 }
 
-}  // namespace tc
-
-// ---------------------------------------------------------------- single-CTA (cta_group::1) variants --
-namespace tc {
-__device__ __forceinline__ void tmem_alloc_cg1(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_cg1() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg1(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma_cg1_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}"
-      :
-      : "r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHi)
-      : "memory");
-}
-__device__ __forceinline__ void commit_cg1(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
 }  // namespace tc

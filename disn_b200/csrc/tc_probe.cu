@@ -238,18 +238,18 @@ __global__ void __launch_bounds__(32, 1) op_cost_kernel(unsigned long long* __re
   MEASURE(lane == 0, { uint32_t ok; asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(db), "r"(0u) : "memory"); acc += ok; });
   // 7: mbarrier.arrive lane 0
   MEASURE(lane == 0, asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bb) : "memory"));
-  // 8: tcgen05.commit (cta_group::1, nothing outstanding), lane 0
-  MEASURE(lane == 0, asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bb) : "memory"));
+  // 8: wgmma.commit_group (nothing outstanding), all lanes
+  MEASURE(true, tc::wgmma_commit());
   // 9: volatile shared load, all lanes (dependent chain through acc)
   MEASURE(true, acc += flag);
-  // 10: tcgen05.fence::after_thread_sync
-  MEASURE(true, tc::tc_fence_after_sync());
+  // 10: wgmma.fence
+  MEASURE(true, tc::wgmma_fence());
   // 11: fence.proxy.async.shared::cta
   MEASURE(true, tc::fence_proxy_async_smem());
   // 12: elect_one + branch
   MEASURE(true, if (tc::elect_one()) acc += 1);
-  // 13: try_wait all lanes followed by tcgen05 fence (the MMA warp's pattern)
-  MEASURE(true, { uint32_t ok; asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(db), "r"(0u) : "memory"); acc += ok; tc::tc_fence_after_sync(); });
+  // 13: try_wait all lanes followed by wgmma.fence (the consumers' pattern)
+  MEASURE(true, { uint32_t ok; asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(db), "r"(0u) : "memory"); acc += ok; tc::wgmma_fence(); });
 #undef MEASURE
   if (acc == 0xFFFFFFFFu) out[63] = acc;
 }
@@ -271,8 +271,8 @@ extern "C" int disn_tc_op_probe(int device) {
   cudaFree(d);
   const char* names[14] = {"empty loop", "try_wait acquire (32 lanes)", "try_wait acquire (1 lane)", "try_wait relaxed (32 lanes)",
                            "try_wait relaxed (1 lane)", "test_wait (32 lanes)", "test_wait (1 lane)", "mbarrier.arrive (1 lane)",
-                           "tcgen05.commit idle (1 lane)", "ld.volatile.shared (32 lanes)", "tcgen05.fence::after_thread_sync",
-                           "fence.proxy.async.shared::cta", "elect.sync + branch", "try_wait + tcgen05 fence (32 lanes)"};
+                           "wgmma.commit_group idle (32 lanes)", "ld.volatile.shared (32 lanes)", "wgmma.fence",
+                           "fence.proxy.async.shared::cta", "elect.sync + branch", "try_wait + wgmma.fence (32 lanes)"};
   for (int i = 0; i < 14; ++i) printf("[op_probe] %-40s %llu cycles/op\n", names[i], h[i]);
   fflush(stdout);
   return 0;

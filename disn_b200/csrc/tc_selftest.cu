@@ -1,8 +1,7 @@
-// Self-test of the tcgen05 cta_group::2 building blocks used by the tensor-core point kernel:
-// one CTA pair computes D[128 x 256] = A[128 x 64] * B[256 x 64]^T (bf16 in, fp32 accumulate) twice
-// (second pass accumulates), exercising TMEM allocation, SW128 K-major descriptors written by threads
-// (A) and by the bulk-copy engine from a host-swizzled image (B), the peer-CTA full-barrier relay,
-// multicast commit, and the 2x2 datapath TMEM layout read back with tcgen05.ld.32x32b.
+// Self-test of the warpgroup-MMA building blocks used by the tensor-core kernels: one warpgroup computes
+// D[128 x 256] = A[128 x 64] * B[256 x 64]^T (bf16 in, fp32 accumulate) as four m64n128 blocks, `passes` times
+// accumulated, exercising SW128 K-major descriptors of tiles written by threads (A) and by the bulk-copy engine from a
+// host-swizzled image (B), and the register layout of the accumulator fragment.
 #include <vector>
 
 #include "common.cuh"
@@ -14,81 +13,65 @@ namespace {
 struct SelfSmem {
   alignas(1024) uint8_t a_tile[64 * 128];     // 64 rows x 64 bf16, SW128
   alignas(1024) uint8_t b_tile[128 * 128];    // 128 rows x 64 bf16, SW128
-  alignas(8) uint64_t b_full;                 // bulk copy of this CTA's B half landed
-  uint64_t peer_full;                         // (leader) peer CTA's operands are ready
-  uint64_t mma_done;                          // accumulators complete (multicast to both CTAs)
-  uint32_t tmem_base;
+  alignas(8) uint64_t b_full;
 };
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(128, 1)
+// D block (c, h) -> D_out[c][64 h + row][col], the layout the test-suite reassembles
+__device__ __forceinline__ void store_block(float* D, int c, int h, const float (&acc)[64]) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int r0 = (tid >> 5) * 16 + (lane >> 2);
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + (lane & 3) * 2 + (i & 1);
+    D[((size_t)c * 128 + h * 64 + row) * 128 + col] = acc[i];
+  }
+}
+
+__global__ void __launch_bounds__(128, 1)
 tc_selftest_kernel(const __nv_bfloat16* __restrict__ A,       // [128][64] row-major
                    const uint8_t* __restrict__ Bimg,          // 2 x 16 KB pre-swizzled halves
-                   float* __restrict__ D,                     // [2 ctas][128 lanes][128 cols]
+                   float* __restrict__ D,                     // [2][128][128]
                    int passes) {
   extern __shared__ uint8_t smem_raw[];
   // dynamic smem is only 16-B aligned by contract: round the shared-window address up to 1024 B
   SelfSmem& s = *reinterpret_cast<SelfSmem*>(smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u));
-  const uint32_t cta = tc::cluster_ctarank();
-  const int tid = threadIdx.x, warp = tid / 32;
-
+  const int tid = threadIdx.x;
   if (tid == 0) {
     tc::mbar_init(&s.b_full, 1);
-    tc::mbar_init(&s.peer_full, 1);
-    tc::mbar_init(&s.mma_done, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 0) {
-    tc::tmem_alloc_cg2(&s.tmem_base, 256);
-    tc::tmem_relinquish_cg2();
-  }
-  // A half of this CTA written by threads exactly like the epilogue will: thread = row, 8 x 16 B chunks
-  if (tid < 64) {
-    const uint4* src = reinterpret_cast<const uint4*>(A + (size_t)(cta * 64 + tid) * 64);
+  __syncthreads();
+  uint32_t phase = 0;
+  for (int c = 0; c < 2; ++c)
+    for (int h = 0; h < 2; ++h) {
+      // A rows of block c written by threads exactly like the epilogues do (thread = row, 8 x 16 B chunks)
+      if (tid < 64) {
+        const uint4* src = reinterpret_cast<const uint4*>(A + (size_t)(c * 64 + tid) * 64);
 #pragma unroll
-    for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(s.a_tile + tc::sw128_offset(tid, c)) = src[c];
-  }
-  tc::fence_proxy_async_smem();
-  tc::tc_fence_before_sync();
-  tc::cluster_sync();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem = s.tmem_base;
-
-  if (tid == 0) {   // B half via the bulk-copy engine
-    tc::mbar_arrive_expect_tx(&s.b_full, 128 * 128);
-    tc::bulk_g2s(s.b_tile, Bimg + (size_t)cta * 128 * 128, 128 * 128, &s.b_full);
-  }
-  if (cta == 1 && tid == 32) {   // relay: tell the leader that this CTA's A (fenced above) and B are in place
-    tc::mbar_wait(&s.b_full, 0);
-    tc::mbar_arrive_cluster(&s.peer_full, 0);
-  }
-  if (cta == 0 && tid == 32) {   // MMA issuer
-    tc::mbar_wait(&s.b_full, 0);
-    tc::mbar_wait_cluster(&s.peer_full, 0);
-    tc::tc_fence_after_sync();
-    const uint32_t idesc = tc::make_idesc_bf16(128, 256);
-    const uint64_t adesc = tc::make_desc_sw128(tc::smem_u32(s.a_tile));
-    const uint64_t bdesc = tc::make_desc_sw128(tc::smem_u32(s.b_tile));
-    for (int p = 0; p < passes; ++p)
-      for (int k = 0; k < 4; ++k)
-        tc::mma_cg2(tmem, tc::desc_advance_k(adesc, k * 16), tc::desc_advance_k(bdesc, k * 16), idesc,
-                    (p | k) ? 1u : 0u);
-    tc::commit_cg2(&s.mma_done, 0b11);
-  }
-  __syncwarp();
-  tc::mbar_wait(&s.mma_done, 0);
-  tc::tc_fence_after_sync();
-  // read back: thread -> lane 32*warp + t, 128 columns
-  const int lane_row = warp * 32 + (tid & 31);
-  for (int c0 = 0; c0 < 128; c0 += 32) {
-    uint32_t r[32];
-    tc::tmem_ld_x32(tmem + ((uint32_t)(warp * 32) << 16) + c0, r);
-    tc::tmem_ld_wait();
+        for (int k = 0; k < 8; ++k) *reinterpret_cast<uint4*>(s.a_tile + tc::sw128_offset(tid, k)) = src[k];
+      }
+      tc::fence_proxy_async_smem();
+      __syncthreads();
+      if (tid == 0) {
+        tc::mbar_arrive_expect_tx(&s.b_full, 128 * 128);
+        tc::bulk_g2s(s.b_tile, Bimg + (size_t)h * 128 * 128, 128 * 128, &s.b_full);
+      }
+      tc::mbar_wait(&s.b_full, phase);
+      phase ^= 1u;
+      float acc[64];
+      tc::acc_fence(acc);
+      tc::wgmma_fence();
+      const uint32_t a0 = tc::smem_u32(s.a_tile), b0 = tc::smem_u32(s.b_tile);
+      for (int p = 0; p < passes; ++p)
 #pragma unroll
-    for (int j = 0; j < 32; ++j) D[((size_t)cta * 128 + lane_row) * 128 + c0 + j] = __uint_as_float(r[j]);
-  }
-  tc::tc_fence_before_sync();
-  tc::cluster_sync();
-  if (warp == 0) tc::tmem_dealloc_cg2(tmem, 256);
+        for (int k = 0; k < 4; ++k)
+          tc::wgmma_m64n128<tc::KIND_BF16>(acc, tc::desc_sw128(a0 + 32u * k), tc::desc_sw128(b0 + 32u * k), (p | k) ? 1u : 0u);
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      tc::acc_fence(acc);
+      store_block(D, c, h, acc);
+      __syncthreads();                        // the tiles are rewritten for the next block
+    }
 }
 
 }  // namespace
@@ -118,7 +101,7 @@ extern "C" int disn_tc_selftest(int device, const float* A, const float* B, int 
   DISN_CUDA_OK(cudaMemset(dD, 0xff, 2 * 128 * 128 * sizeof(float)));
   DISN_CUDA_OK(cudaFuncSetAttribute(tc_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)sizeof(SelfSmem) + 1024));
-  tc_selftest_kernel<<<2, 128, sizeof(SelfSmem) + 1024>>>(dA, dB, dD, passes);
+  tc_selftest_kernel<<<1, 128, sizeof(SelfSmem) + 1024>>>(dA, dB, dD, passes);
   DISN_CUDA_OK(cudaGetLastError());
   DISN_CUDA_OK(cudaDeviceSynchronize());
   DISN_CUDA_OK(cudaMemcpy(D_out, dD, 2 * 128 * 128 * sizeof(float), cudaMemcpyDeviceToHost));
@@ -127,9 +110,10 @@ extern "C" int disn_tc_selftest(int device, const float* A, const float* B, int 
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Mixed-kind self-test (building block of DISN_PREC_F16F8): one accumulator receives
-//   D = fp16(A16) * fp16(B16)^T   (kind::f16, SW128 tiles, 4 x K=16)
-//     + e5m2(A8) * e5m2(B8)^T     (kind::f8f6f4, SW64 tiles of bytes, 2 x K=32)
+// Mixed-kind self-test (building block of DISN_PREC_F16F8):
+//   D = fp16(A16) * fp16(B16)^T   (SW128 tiles, 4 x K=16, main accumulator)
+//     + e5m2(A8) * e5m2(B8)^T     (SW64 tiles of bytes, 2 x K=32, zero-initialised second accumulator added in fp32,
+//                                  as the point kernel does)
 // mode bit 0 enables the f16 part, bit 1 the f8 part.
 // ---------------------------------------------------------------------------------------------------------
 #include <cuda_fp16.h>
@@ -144,85 +128,72 @@ struct MixSmem {
   alignas(1024) uint8_t a8[64 * 64];
   alignas(1024) uint8_t b8[128 * 64];
   alignas(8) uint64_t b_full;
-  uint64_t peer_full;
-  uint64_t mma_done;
-  uint32_t tmem_base;
 };
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(128, 1)
+__global__ void __launch_bounds__(128, 1)
 tc_selftest_mixed_kernel(const __half* __restrict__ A16, const uint8_t* __restrict__ A8,      // [128][64] row-major
-                         const uint8_t* __restrict__ Bimg,   // per CTA: 16 KB SW128 fp16 + 8 KB SW64 e5m2
+                         const uint8_t* __restrict__ Bimg,   // per 128-row half: 16 KB SW128 fp16 + 8 KB SW64 e5m2
                          float* __restrict__ D, int mode) {
   extern __shared__ uint8_t smem_raw[];
   MixSmem& s = *reinterpret_cast<MixSmem*>(smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u));
-  const uint32_t cta = tc::cluster_ctarank();
-  const int tid = threadIdx.x, warp = tid / 32;
+  const int tid = threadIdx.x;
   if (tid == 0) {
     tc::mbar_init(&s.b_full, 1);
-    tc::mbar_init(&s.peer_full, 1);
-    tc::mbar_init(&s.mma_done, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 0) {
-    tc::tmem_alloc_cg2(&s.tmem_base, 256);
-    tc::tmem_relinquish_cg2();
-  }
-  if (tid < 64) {
-    const uint4* src = reinterpret_cast<const uint4*>(A16 + (size_t)(cta * 64 + tid) * 64);
+  __syncthreads();
+  uint32_t phase = 0;
+  for (int c = 0; c < 2; ++c)
+    for (int h = 0; h < 2; ++h) {
+      if (tid < 64) {
+        const uint4* src = reinterpret_cast<const uint4*>(A16 + (size_t)(c * 64 + tid) * 64);
 #pragma unroll
-    for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(s.a16 + tc::sw128_offset(tid, c)) = src[c];
-    const uint4* src8 = reinterpret_cast<const uint4*>(A8 + (size_t)(cta * 64 + tid) * 64);
+        for (int k = 0; k < 8; ++k) *reinterpret_cast<uint4*>(s.a16 + tc::sw128_offset(tid, k)) = src[k];
+        const uint4* src8 = reinterpret_cast<const uint4*>(A8 + (size_t)(c * 64 + tid) * 64);
 #pragma unroll
-    for (int c = 0; c < 4; ++c) *reinterpret_cast<uint4*>(s.a8 + tc::sw64_offset(tid, c)) = src8[c];
-  }
-  tc::fence_proxy_async_smem();
-  tc::tc_fence_before_sync();
-  tc::cluster_sync();
-  tc::tc_fence_after_sync();
-  const uint32_t tmem = s.tmem_base;
-  if (tid == 0) {
-    tc::mbar_arrive_expect_tx(&s.b_full, 128 * 128 + 128 * 64);
-    tc::bulk_g2s(s.b16, Bimg + (size_t)cta * (128 * 192), 128 * 128, &s.b_full);
-    tc::bulk_g2s(s.b8, Bimg + (size_t)cta * (128 * 192) + 128 * 128, 128 * 64, &s.b_full);
-  }
-  if (cta == 1 && tid == 32) {
-    tc::mbar_wait(&s.b_full, 0);
-    tc::mbar_arrive_cluster(&s.peer_full, 0);
-  }
-  if (cta == 0 && tid == 32) {
-    tc::mbar_wait(&s.b_full, 0);
-    tc::mbar_wait_cluster(&s.peer_full, 0);
-    tc::tc_fence_after_sync();
-    const uint32_t a16 = tc::desc_lo(tc::smem_u32(s.a16)), b16 = tc::desc_lo(tc::smem_u32(s.b16));
-    const uint32_t a8 = tc::desc_lo(tc::smem_u32(s.a8)), b8 = tc::desc_lo(tc::smem_u32(s.b8));
-    uint32_t acc = 0;
-    if (mode & 1)
-      for (int k = 0; k < 4; ++k) { tc::mma_cg2_lo(tmem, a16 + 2u * k, b16 + 2u * k, tc::make_idesc_f16(128, 256), acc); acc = 1; }
-    if (mode & 2)
-      for (int k = 0; k < 2; ++k) { tc::mma_cg2_f8_lo(tmem, a8 + 2u * k, b8 + 2u * k, tc::make_idesc_e5m2(128, 256), acc); acc = 1; }
-    tc::commit_cg2(&s.mma_done, 0b11);
-  }
-  __syncwarp();
-  tc::mbar_wait(&s.mma_done, 0);
-  tc::tc_fence_after_sync();
-  const int lane_row = warp * 32 + (tid & 31);
-  for (int c0 = 0; c0 < 128; c0 += 32) {
-    uint32_t r[32];
-    tc::tmem_ld_x32(tmem + ((uint32_t)(warp * 32) << 16) + c0, r);
-    tc::tmem_ld_wait();
+        for (int k = 0; k < 4; ++k) *reinterpret_cast<uint4*>(s.a8 + tc::sw64_offset(tid, k)) = src8[k];
+      }
+      tc::fence_proxy_async_smem();
+      __syncthreads();
+      if (tid == 0) {
+        tc::mbar_arrive_expect_tx(&s.b_full, 128 * 128 + 128 * 64);
+        tc::bulk_g2s(s.b16, Bimg + (size_t)h * (128 * 192), 128 * 128, &s.b_full);
+        tc::bulk_g2s(s.b8, Bimg + (size_t)h * (128 * 192) + 128 * 128, 128 * 64, &s.b_full);
+      }
+      tc::mbar_wait(&s.b_full, phase);
+      phase ^= 1u;
+      float acc[64], cor[64];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) D[((size_t)cta * 128 + lane_row) * 128 + c0 + j] = __uint_as_float(r[j]);
-  }
-  tc::tc_fence_before_sync();
-  tc::cluster_sync();
-  if (warp == 0) tc::tmem_dealloc_cg2(tmem, 256);
+      for (int i = 0; i < 64; ++i) acc[i] = cor[i] = 0.f;
+      tc::acc_fence(acc);
+      tc::acc_fence(cor);
+      tc::wgmma_fence();
+      if (mode & 1)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          tc::wgmma_m64n128<tc::KIND_F16>(acc, tc::desc_sw128(tc::smem_u32(s.a16) + 32u * k),
+                                          tc::desc_sw128(tc::smem_u32(s.b16) + 32u * k), k ? 1u : 0u);
+      if (mode & 2)
+#pragma unroll
+        for (int k = 0; k < 2; ++k)
+          tc::wgmma_m64n128<tc::KIND_E5M2>(cor, tc::desc_sw64(tc::smem_u32(s.a8) + 32u * k),
+                                           tc::desc_sw64(tc::smem_u32(s.b8) + 32u * k), k ? 1u : 0u);
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      tc::acc_fence(acc);
+      tc::acc_fence(cor);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] += cor[i];
+      store_block(D, c, h, acc);
+      __syncthreads();
+    }
 }
 
 }  // namespace
 }  // namespace disn
 
 // Host fp32 inputs A16,A8 [128*64], B16,B8 [256*64]; the e5m2 roundings actually used are returned in A8q/B8q so the
-// caller can form the exact reference.  D_out [2*128*128] in TMEM (cta, lane, column) order.
+// caller can form the exact reference.  D_out [2*128*128]: D_out[c][64 h + r][j] = D[64 c + r][128 h + j].
 extern "C" int disn_tc_selftest_mixed(int device, const float* A16, const float* B16, const float* A8, const float* B8,
                                       int mode, float* A8q, float* B8q, float* D_out) {
   using namespace disn;
@@ -255,7 +226,7 @@ extern "C" int disn_tc_selftest_mixed(int device, const float* A16, const float*
   DISN_CUDA_OK(cudaDeviceSynchronize());
   DISN_CUDA_OK(cudaFuncSetAttribute(tc_selftest_mixed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)sizeof(MixSmem) + 1024));
-  tc_selftest_mixed_kernel<<<2, 128, sizeof(MixSmem) + 1024>>>(dA, dA8, dB, dD, mode);
+  tc_selftest_mixed_kernel<<<1, 128, sizeof(MixSmem) + 1024>>>(dA, dA8, dB, dD, mode);
   DISN_CUDA_OK(cudaGetLastError());
   DISN_CUDA_OK(cudaDeviceSynchronize());
   DISN_CUDA_OK(cudaMemcpy(D_out, dD, 2 * 128 * 128 * sizeof(float), cudaMemcpyDeviceToHost));

@@ -1,5 +1,5 @@
 """Mirror of the reference's single-image demo (demo/demo.py): one 137x137 render -> (optionally estimated) camera ->
-dense SDF grid -> mesh, on the B200 path.  Same function names and argument meaning as the reference's module:
+dense SDF grid -> mesh, on the CUDA path.  Same function names and argument meaning as the reference's module:
 
     read_img_get_transmat()      demo/demo.py:261-279   image -> batch_data {img, trans_mat, sdf_params}
     cam_evl(img_arr)             demo/demo.py:195-258   estimated-camera network -> pred_trans_mat

@@ -1,5 +1,5 @@
 """Drop-in mirror of the reference's ``models/model_normalization.py`` call surface for the SDF-inference
-hot path (twostream, non-binary branch), executed by the B200 C-ABI library instead of a TF-1.x graph.
+hot path (twostream, non-binary branch), executed by the C-ABI library instead of a TF-1.x graph.
 
 Same function names, argument meaning and end_points keys as the reference
 (models/model_normalization.py:14 placeholder_inputs, :38 placeholder_features, :47 get_model,
@@ -81,7 +81,7 @@ def _check_flags(FLAGS):
     for flag in ("binary", "threedcnn", "img_feat_onestream", "multi_view", "alpha"):
         if getattr(FLAGS, flag, False):
             raise NotImplementedError("FLAGS.%s selects an ablation branch of the reference graph that is outside "
-                                      "the B200 hot path (SURVEY.md section 2)" % flag)
+                                      "the CUDA hot path (SURVEY.md section 2)" % flag)
     if not getattr(FLAGS, "img_feat_twostream", False):
         raise NotImplementedError("only the --img_feat_twostream graph (the DISN model) is implemented")
 

@@ -1,6 +1,6 @@
 """Mirror of the two reference MLP heads on the hot path (models/sdfnet.py:69-92 get_sdf_basic2,
 :171-190 get_sdf_basic2_imgfeat_twostream).  In the reference these build 1x1-conv sub-graphs inside
-get_model; on the B200 path both heads live inside the fused point kernel.  Called on their own -- with placeholders
+get_model; on the CUDA path both heads live inside the fused point kernel.  Called on their own -- with placeholders
 (symbolic, evaluated by Session.run) or with arrays (eager, on the engine given to set_engine) -- they run one stream of that
 kernel through the explicit-feature entry point (disn_eval_features).
 

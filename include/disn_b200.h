@@ -1,5 +1,5 @@
 /*
- * disn_b200.h -- C ABI of the B200-native DISN SDF-inference hot path.
+ * disn_b200.h -- C ABI of the H100-native (sm_90a) DISN SDF-inference hot path.
  *
  * The reference has no FFI on this path (it is a Python-built TF-1.x graph); the entry points
  * below are what a replacement of that graph binds, one per reference call site
@@ -46,8 +46,8 @@ enum {
 /* arithmetic used by the fused point kernel */
 enum {
   DISN_PREC_FP32 = 0,    /* CUDA-core fp32 FMA (exact restatement of the reference arithmetic) */
-  DISN_PREC_BF16X3 = 1,  /* tcgen05 tensor cores, bf16 hi/lo split operands, 3 MMAs per product, fp32 accumulate */
-  DISN_PREC_F16F8 = 2,   /* tcgen05: fp16 main product + two e5m2 (kind::f8f6f4, 2x rate) correction products, fp32
+  DISN_PREC_BF16X3 = 1,  /* tensor cores (wgmma), bf16 hi/lo split operands, 3 MMAs per product, fp32 accumulate */
+  DISN_PREC_F16F8 = 2,   /* wgmma: fp16 main product + two e5m2 (2x rate) correction products, fp32
                             accumulate: 2 MMA-units per product instead of 3; activations must stay below 65504 */
 };
 

@@ -1,4 +1,4 @@
-/* Diagnostics of the DISN B200 library: building blocks, probes and debug harnesses used by tests/ and tools/.
+/* Diagnostics of the DISN library: building blocks, probes and debug harnesses used by tests/ and tools/.
  * They live in libdisn_b200_test.so (the product library libdisn_b200.so does not export them). */
 #ifndef DISN_B200_TEST_H
 #define DISN_B200_TEST_H
@@ -7,23 +7,23 @@
 extern "C" {
 #endif
 
-/* Diagnostic: one CTA-pair tcgen05 (cta_group::2) GEMM D[128x256] = A[128x64] * B[256x64]^T, `passes` times
- * accumulated; returns the raw TMEM image D_out[2 CTAs][128 lanes][128 columns]. Host pointers. */
+/* Diagnostic: one warpgroup-MMA GEMM D[128x256] = A[128x64] * B[256x64]^T (bf16, four m64n128 blocks), `passes` times
+ * accumulated; D_out[c][64h + r][j] = D[64c + r][128h + j] (c, h in {0,1}). Host pointers. */
 int disn_tc_selftest(int device, const float* A, const float* B, int passes, float* D_out);
 /* Diagnostic: mixed-kind accumulation used by DISN_PREC_F16F8 -- D = fp16(A16).fp16(B16)^T (mode bit 0) +
- * e5m2(A8).e5m2(B8)^T (mode bit 1) into one TMEM accumulator; A8q/B8q return the e5m2 values actually used. */
+ * e5m2(A8).e5m2(B8)^T (mode bit 1) summed in fp32, D_out laid out as above; A8q/B8q return the e5m2 values actually used. */
 int disn_tc_selftest_mixed(int device, const float* A16, const float* B16, const float* A8, const float* B8, int mode,
                            float* A8q, float* B8q, float* D_out);
 
 /* Diagnostic: one encoder GEMM (plain when H == 0, else the 3x3 SAME im2col view of NHWC A[M/(H*W),H,W,Cin]) through
- * the fp32 CUDA-core kernel and through the tcgen05 kernel; host pointers, outputs [M,N]. */
+ * the fp32 CUDA-core kernel and through the tensor-core kernel; host pointers, outputs [M,N]. */
 int disn_debug_gemm(disn_ctx* ctx, const float* A, const float* Wt, const float* bias, int M, int N, int K, int H, int W,
                     int Cin, int relu, float* out_fp32, float* out_tc);
 
 /* Diagnostic: prints the achievable L2 -> shared-memory bulk-copy streaming rate (bytes/clk/SM) for a sweep of
  * ring depths, stage sizes and cluster multicast widths (the weight-streaming pattern of the tensor-core kernel). */
 int disn_tc_stream_probe(int device);
-/* Diagnostic: prints the issue cost (cycles) of the mbarrier / tcgen05 synchronisation instructions of the MMA warp. */
+/* Diagnostic: prints the issue cost (cycles) of the mbarrier / wgmma synchronisation instructions of the consumers. */
 int disn_tc_op_probe(int device);
 
 #ifdef __cplusplus

@@ -127,12 +127,12 @@ def test_config0_res64_grid_vs_oracle(eng8, he_weights, oracle_enc8, init):
 
 
 def test_config2_batch8_res128_grid_vs_oracle(eng8, he_weights, oracle_enc8):
-    """BASELINE config 2 (batch of 8 renders, --sdf_res 128 -> 8 x 129^3 points, VGG on tcgen05): every image of the
+    """BASELINE config 2 (batch of 8 renders, --sdf_res 128 -> 8 x 129^3 points, VGG on the tensor cores): every image of the
     batch against the float64 oracle at 2 500 sampled indices (20 000 in total), ShapeNet-style cameras and boxes."""
     imgs, enc = oracle_enc8
     eng8.set_precision("f16f8")
     eng8.encode(imgs)
-    # encoder products of the batch (tcgen05 conv path) vs the oracle
+    # encoder products of the batch (tensor-core conv path) vs the oracle
     emb = eng8.get_encoded(0)
     assert np.abs(emb - enc.img_embedding).max() <= 2e-4 * np.abs(enc.img_embedding).max()   # measured 6e-5 (bf16x3 convs, split-K)
     tm = synth.synthetic_trans_mats(8, seed=4321)

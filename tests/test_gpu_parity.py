@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path through the C ABI against the CPU oracle
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C ABI against the CPU oracle
 on the same seeded inputs.  Tolerance (BASELINE.json north_star): |sdf_gpu - sdf_ref| <= 1e-4 abs on the
 SDF value (= pred/10), i.e. 1e-3 on pred; the fp32 path is held to 10x tighter."""
 import numpy as np

@@ -33,7 +33,7 @@ def test_broken_protocols_are_detected(mutation):
 
 
 def test_dual_issuer_variant_is_sound():
-    """The protocol of profiles/r01f_experiment_dual_issuer.diff (one MMA warp per N-block, producers owning fixed slots,
+    """The dual-issuer protocol variant (one MMA warp per N-block, producers owning fixed slots,
     every waiter observing every phase) -- the variant the round-2 plan builds on -- with 3 and 4 weight slots."""
     for prm in ({"issuers": 2, "NW": 3}, {"issuers": 2, "NW": 4, "split_wfull": 1}):
         for seed in range(15):

@@ -1,6 +1,6 @@
 """Same-GPU, same-process A/B of the fused point kernel under different environment switches.
 
-    python tools/kbench.py [--res 256] [--precision f16f8] [--reps 5] [--rounds 2] "DISN_TC_VAR=0" "DISN_TC_VAR=16,DISN_TC_EXPT=6" ...
+    python tools/kbench.py [--res 256] [--precision f16f8] [--reps 5] [--rounds 2] "DISN_TC_CORR=0xFF" "DISN_TC_CORR=0xDF" ...
 
 The C library reads its switches with getenv() at launch time, so one process (weights loaded once, image encoded once) can
 interleave all configurations.  Prints the mean kernel time per configuration and round (CUDA events on the launching stream).

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (raw page) or an ncu launch-list CSV into the text files kept under profiles/.
-    python tools/ncu_summary.py raw  gpurun_out/x.ncu-rep   > profiles/x_ncu.txt
-    python tools/ncu_summary.py list gpurun_out/launches.csv > profiles/x_launches.txt
+"""Summarise an .ncu-rep (raw page) or an ncu launch-list CSV into text summaries.
+    python tools/ncu_summary.py raw  x.ncu-rep > x_ncu.txt
+    python tools/ncu_summary.py list launches.csv > x_launches.txt
 """
 import collections
 import csv

@@ -1,24 +1,22 @@
 #!/usr/bin/env python
-"""Discrete-event model of the synchronisation protocol of point_tc_kernel (disn_b200/csrc/point_tc.cu).
+"""Discrete-event model of the synchronisation protocol of a warp-specialised variant of the fused point kernel: a CTA pair
+sharing tensor-memory accumulators, weight-producer warps, one or two MMA issuer warps, two epilogue groups and a front end.
+It is not the protocol of the shipped kernel (disn_b200/csrc/point_tc.cu, two consumer warpgroups with register
+accumulators); it is kept as a checker for that deeper pipeline organisation.
 
 Why: on the GPU a protocol bug is a 4-second trap or silent corruption and costs a scarce GPU run; most of them (dead-
 locks, a parity wait by an agent that skipped a phase, a ring slot overwritten before it was consumed, an accumulator
 overwritten while it is still being drained) are properties of the *protocol*, not of the hardware.  This model runs
-the same agents -- weight producers, MMA issuer, two epilogue groups, front end -- as Python generators over mbarrier
-objects with the hardware's semantics (arrival counts, phases, parity waits that can alias), under randomised operation
-latencies, and checks:
+the agents as Python generators over mbarrier objects with the hardware's semantics (arrival counts, phases, parity waits
+that can alias), under randomised operation latencies, and checks:
   * no deadlock (every agent terminates);
   * every successful parity wait observed exactly the phase the agent meant (no aliasing, no overrun);
   * every MMA reads the weight stage / activation slice it expects (ring contents are versioned);
   * no accumulator region is written while an overlapping older accumulator still has undrained slices.
 One CTA of the pair is modelled (arrival counts that come from both CTAs are halved; the peer adds latency only).
 
-It doubles as a coarse performance model: the operation costs in PARAMS start from the ones measured on B200 (DESIGN.md
-4.1: op-cost probe, wait traces, one-tile timeline) and are tuned so that the model reproduces the measured cycles per tile
-and blocked-time split of ROUND 1's kernel within ~10 % (f16f8: 58.7 K vs 59.9 K measured; the shipped round-2 kernel is the
-variant --set x2_in_ring=1 --set NW=4 --set issuers=2 --set split_wfull=1, measured at 54.3 K), `report()` prints cycles per tile and
-the per-agent blocked time in the same classes as the DISN_TC_MEASURE build, and `--set key=value` / `--mode` explore what-ifs (ring depths, operand mode, faster
-epilogue ...) before spending GPU time on them.
+The operation costs in PARAMS are nominal cycle counts, not measurements; `report()` prints modelled cycles per tile and
+the per-agent blocked time, and `--set key=value` / `--mode` explore what-ifs (ring depths, operand mode, ...).
 
     python tools/tc_protocol_sim.py [--tiles N] [--schedules N] [--mode f16f8|bf16x3] [--set key=value ...] [--report]
 """
@@ -36,7 +34,7 @@ PARAMS = dict(
                        #     the front end publishes), freeing the dedicated 16 KB slot for a fourth weight stage
     split_wfull=0,     # issuers=2 only: 1 = one 'stage landed' barrier per (issuer, slot), signalled according to the static
                        #     stage -> issuer map, so that an issuer only ever waits on barriers whose every phase is its own
-    issuers=1,         # 2 = the dual-issuer experiment (profiles/r01f_experiment_dual_issuer.diff): one MMA warp per N-block,
+    issuers=1,         # 2 = the dual-issuer variant: one MMA warp per N-block,
                        #     producers with fixed slot ownership that do not wait for the data, peer relay warp
     op=100,            # an mbarrier try_wait that succeeds at once / an arrive, on a busy SM
     commit=150,        # tcgen05.commit
