@@ -56,6 +56,9 @@ EXPORTS = {
                               C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "disn_mc_fetch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "disn_mc_write_obj": (C.c_int, [C.c_void_p, C.c_char_p]),
+    "disn_mesh_load": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]),
+    "disn_mesh_clean": (C.c_int, [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.POINTER(C.c_int64),
+                                  C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "disn_fetch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]),
     "disn_shared_alloc": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_void_p), C.c_char_p]),
     "disn_shared_open": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

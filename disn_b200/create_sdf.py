@@ -127,6 +127,8 @@ def test_one_epoch(sess, ops, batches):
     (disn_eval_grid_resident), then per image the CUDA marching-cubes post-pass straight on that buffer and the OBJ writer
     (formatted on a worker thread, like the reference's 4-worker pool for its mesher, create_sdf.py:238,288).
     No .dist round trip through the file system; FLAGS.keep_dist=True also writes the reference's .dist artefact.
+    FLAGS.clean_smallparts=True runs the reference's postprocessing/clean_smallparts.py step on each mesh while it is
+    still in HBM (thresholds FLAGS.clean_dist_thresh / clean_num_thresh, default 0.5 / 0.3).
     The reference's literal loop (host grid, SPLIT_SIZE chunks through sess.run, reassembly, /SDF_WEIGHT) is kept as a
     verification aid in tests/reference_loop.py."""
     log_string(str(datetime.now()))
@@ -144,8 +146,15 @@ def test_one_epoch(sess, ops, batches):
                                                                        batch_data["obj_nm"][b], batch_data["view_id"][b]))
                     path = obj_path(RESULT_OBJ_PATH, batch_data["cat_id"][b], batch_data["obj_nm"][b], batch_data["view_id"][b])
                     dev = grid_ptr + b * R * R * R * 4
-                    verts, faces = sess.engine.marching_cubes(None, batch_data["sdf_params"][b], float(FLAGS.iso),
-                                                              device_ptr=dev, R=R)
+                    if getattr(FLAGS, "clean_smallparts", False):
+                        # postprocessing/clean_smallparts.py on the resident mesh before it leaves HBM
+                        sess.engine.marching_cubes(None, batch_data["sdf_params"][b], float(FLAGS.iso), device_ptr=dev,
+                                                   R=R, fetch=False)
+                        verts, faces = sess.engine.clean_mesh(getattr(FLAGS, "clean_dist_thresh", 0.5),
+                                                              getattr(FLAGS, "clean_num_thresh", 0.3))
+                    else:
+                        verts, faces = sess.engine.marching_cubes(None, batch_data["sdf_params"][b], float(FLAGS.iso),
+                                                                  device_ptr=dev, R=R)
                     if getattr(FLAGS, "keep_dist", False):
                         to_binary(R - 1, batch_data["sdf_params"][b], sess.engine.fetch(dev, (R, R, R)), path[:-4] + ".dist")
                     futures.append(executor.submit(_write_and_return, path, verts, faces))
@@ -197,6 +206,26 @@ def write_obj(path, verts, faces):
     f = np.ascontiguousarray(faces, np.int32)
     _lib.check(_lib.load().disn_write_obj(path.encode(), v.ctypes.data_as(C.c_void_p), len(v),
                                           f.ctypes.data_as(C.c_void_p), len(f)))
+
+
+def read_obj(path):
+    """Triangle mesh of an OBJ file: `v x y z` records and `f` records of `i`, `i/j` or `i/j/k` tokens (1-based) ->
+    (verts [V,3] float32, faces [F,3] int32 0-based).  Other record types are ignored; a face that is not a triangle
+    raises ValueError."""
+    verts, faces = [], []
+    with open(path) as fh:
+        for n, line in enumerate(fh, 1):
+            tok = line.split()
+            if not tok:
+                continue
+            if tok[0] == "v":
+                verts.append([float(x) for x in tok[1:4]])
+            elif tok[0] == "f":
+                if len(tok) != 4:
+                    raise ValueError("%s:%d: only triangle faces are supported, found %d corners" % (path, n, len(tok) - 1))
+                faces.append([int(t.split("/")[0]) - 1 for t in tok[1:]])
+    return (np.array(verts, np.float64).astype(np.float32).reshape(-1, 3),
+            np.array(faces, np.int64).astype(np.int32).reshape(-1, 3))
 
 
 def create_one_cube_obj(marching_cube_command, i, sdf_file, cube_obj_file):

@@ -76,6 +76,7 @@ void disn_destroy(disn_ctx* c) {
   if (c->tc_weights_f8) cudaFree(c->tc_weights_f8);
   if (c->d_status) cudaFree(c->d_status);
   mc_free(c);
+  mesh_clean_free(c);
   if (c->d_grid) cudaFree(c->d_grid);
   if (c->d_mc_in) cudaFree(c->d_mc_in);
   if (c->nn_scratch) cudaFree(c->nn_scratch);
@@ -517,6 +518,19 @@ int disn_marching_cubes(disn_ctx* c, const float* sdf, int32_t R, const double* 
   if (*n_verts < nv || *n_faces < nf) { set_error("marching_cubes: output buffers too small"); return -2; }
   *n_verts = nv; *n_faces = nf;
   return mc_fetch(c, verts, faces);
+}
+
+int disn_mesh_load(disn_ctx* c, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces) {
+  DISN_REQUIRE(c, "null ctx");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  return mesh_load(c, verts, n_verts, faces, n_faces);
+}
+
+int disn_mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
+                    int64_t* n_kept, int64_t* n_verts, int64_t* n_faces) {
+  DISN_REQUIRE(c, "null ctx");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  return mesh_clean(c, dist_thresh, num_thresh, face_component, n_components, n_kept, n_verts, n_faces);
 }
 
 int disn_eval_grid_resident(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t B, int32_t sdf_res,

@@ -141,6 +141,11 @@ struct disn_ctx {
   uint32_t* mc_totals = nullptr; uint32_t* mc_totals_host = nullptr;
   float* mc_verts = nullptr; int32_t* mc_faces = nullptr;
   int64_t mc_pts_cap = 0, mc_verts_cap = 0, mc_faces_cap = 0, mc_nv = 0, mc_nf = 0;
+  // small-part cleaning of the resident mesh (mesh_clean.cu): scratch arena, the compacted mesh's buffers (swapped with
+  // mc_verts / mc_faces after a clean) and the totals read back once per clean; all grow only
+  void* cl_arena = nullptr; int64_t cl_arena_bytes = 0;
+  float* cl_verts = nullptr; int32_t* cl_faces = nullptr; int64_t cl_verts_cap = 0, cl_faces_cap = 0;
+  uint32_t* cl_totals_host = nullptr;
   // device-resident SDF grid of disn_eval_grid_resident and host staging for the marching-cubes input
   float* d_grid = nullptr; int64_t grid_cap = 0;
   float* d_mc_in = nullptr; int64_t mc_in_cap = 0;
@@ -181,4 +186,12 @@ int nn_distance(disn_ctx* c, const float* d_xyz1, int n, const float* d_xyz2, in
 int mc_run(disn_ctx* c, const float* d_sdf, int R, const double* bbox, float iso, int64_t* n_verts, int64_t* n_faces);
 int mc_fetch(disn_ctx* c, float* verts, int32_t* faces);
 void mc_free(disn_ctx* c);
+// in-place exclusive scan of d[0..n) on c->stream, total -> *d_total (device); `sums` = scan_scratch_elems(n) words
+int64_t scan_scratch_elems(int64_t n);
+int exclusive_scan(disn_ctx* c, uint32_t* d, int64_t n, uint32_t* d_total, uint32_t* sums);
+// mesh_clean.cu
+int mesh_load(disn_ctx* c, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces);
+int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
+               int64_t* n_kept, int64_t* n_verts, int64_t* n_faces);
+void mesh_clean_free(disn_ctx* c);
 }  // namespace disn

@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
+from typing import NamedTuple
 
 import numpy as np
 
@@ -15,6 +16,14 @@ TAP_C = (64, 128, 256, 512, 512)
 
 def _f32(a):
     return np.ascontiguousarray(a, dtype=np.float32)
+
+
+class MeshCleanCounts(NamedTuple):
+    """Result counts of Engine.clean_mesh: the cleaned mesh's size, the components found and the components kept."""
+    n_verts: int
+    n_faces: int
+    n_components: int
+    n_kept: int
 
 
 class Engine:
@@ -34,6 +43,8 @@ class Engine:
         self._h = C.c_void_p()
         check(self.lib.disn_create(C.byref(cfg), C.byref(self._h)))
         self.batch = 0
+        self._mesh_faces = 0        # face count of the resident mesh (sizes clean_mesh's labels)
+        self.last_clean = None
 
     # -- lifetime -----------------------------------------------------------------------------
     def close(self):
@@ -287,6 +298,7 @@ class Engine:
             ptr, flags = C.c_void_p(device_ptr), DISN_DEVICE_PTR
         nv, nf = C.c_int64(0), C.c_int64(0)
         check(self.lib.disn_mc_run(self._h, ptr, R, bb, float(iso), flags, C.byref(nv), C.byref(nf)))
+        self._mesh_faces = nf.value
         if not fetch:
             return nv.value, nf.value
         verts = np.empty((nv.value, 3), dtype=np.float32)
@@ -296,8 +308,36 @@ class Engine:
         return verts, faces
 
     def write_mesh_obj(self, path: str):
-        """OBJ of the mesh left in HBM by the last marching_cubes call (reference mesher's output conventions)."""
+        """OBJ of the mesh left in HBM by the last marching_cubes / load_mesh / clean_mesh call (reference mesher's output
+        conventions)."""
         check(self.lib.disn_mc_write_obj(self._h, path.encode()))
+
+    def load_mesh(self, verts, faces):
+        """Upload a mesh (verts [V,3] float32, faces [F,3] 0-based) into the resident slot marching_cubes fills."""
+        v = _f32(verts).reshape(-1, 3)
+        f = np.ascontiguousarray(faces, np.int32).reshape(-1, 3)
+        check(self.lib.disn_mesh_load(self._h, v.ctypes.data_as(C.c_void_p), len(v), f.ctypes.data_as(C.c_void_p), len(f)))
+        self._mesh_faces = len(f)
+
+    def clean_mesh(self, dist_thresh: float = 0.5, num_thresh: float = 0.3, fetch: bool = True, want_labels: bool = False):
+        """postprocessing/clean_smallparts.py:38-54 on the resident mesh, in place: drop every edge-connected component
+        with n_c <= max n_c * num_thresh vertices or a centroid at distance >= dist_thresh from the origin.
+        -> (verts, faces), plus the per-face component labels of the input mesh if want_labels; fetch=False returns
+        the MeshCleanCounts instead of the mesh (and the labels).  The counts of the last call are in `last_clean`."""
+        labels = np.empty(self._mesh_faces, np.int32) if want_labels else None
+        nc, nk, nv, nf = (C.c_int64(0) for _ in range(4))
+        check(self.lib.disn_mesh_clean(self._h, float(dist_thresh), float(num_thresh),
+                                       None if labels is None else labels.ctypes.data_as(C.c_void_p),
+                                       C.byref(nc), C.byref(nk), C.byref(nv), C.byref(nf)))
+        self._mesh_faces = nf.value
+        self.last_clean = MeshCleanCounts(nv.value, nf.value, nc.value, nk.value)
+        if not fetch:
+            return (self.last_clean, labels) if want_labels else self.last_clean
+        verts = np.empty((nv.value, 3), dtype=np.float32)
+        faces = np.empty((nf.value, 3), dtype=np.int32)
+        if nv.value and nf.value:
+            check(self.lib.disn_mc_fetch(self._h, verts.ctypes.data_as(C.c_void_p), faces.ctypes.data_as(C.c_void_p)))
+        return (verts, faces, labels) if want_labels else (verts, faces)
 
     def eval_grid_resident(self, sdf_params, trans_mat, sdf_res: int) -> int:
         """Whole [B,R,R,R] grid evaluated into the context's HBM buffer; returns its device address."""

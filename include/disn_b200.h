@@ -20,6 +20,8 @@
  *   disn_write_dist                 <-> to_binary (test/create_sdf.py:292-303)
  *   disn_marching_cubes(+_to_obj)   <-> os.system("./isosurface/computeMarchingCubes <dist> <obj> -i <iso>")
  *                                       (test/create_sdf.py:319-323)
+ *   disn_mesh_load / disn_mesh_clean <-> clean_single_mesh (postprocessing/clean_smallparts.py:38-54):
+ *                                       pymesh.separate_mesh, keep rule, pymesh.merge_meshes
  *
  * Conventions: every function returns 0 on success, non-zero on failure with a thread-local message
  * in disn_last_error(); the caller owns all buffers; all tensors are float32, row-major, NHWC / [B,N,C]
@@ -129,6 +131,22 @@ int disn_mc_run(disn_ctx* ctx, const float* sdf, int32_t R, const double* bbox, 
 int disn_mc_fetch(disn_ctx* ctx, float* verts, int32_t* faces);
 int disn_mc_write_obj(disn_ctx* ctx, const char* path);
 int disn_fetch(disn_ctx* ctx, const void* dev, void* host, int64_t bytes);
+
+/* Small-part removal, the reference's clean_single_mesh (postprocessing/clean_smallparts.py:38-54), on the resident mesh
+ * of disn_mc_run / disn_mesh_load; disn_mc_fetch and disn_mc_write_obj then return the cleaned mesh.
+ *   disn_mesh_load: uploads a host mesh (verts [n_verts,3] float32, faces [n_faces,3] int32 0-based) into that slot; a
+ *     face index outside [0, n_verts) is an error.
+ *   disn_mesh_clean: components = faces connected through shared undirected edges {a,b}, a != b (PyMesh "face"
+ *     connectivity), numbered in order of their smallest face; n_c = distinct vertices of component c; centroid from
+ *     fixed-point sums (round(v * 2^32) in int64); keep c iff n_c > max n_c * num_thresh and |centroid| < dist_thresh
+ *     (the reference uses 0.5 / 0.3).  The result holds the kept faces and the vertices they reference, both in their
+ *     original order (a vertex shared by two kept components appears once).  face_component: NULL or host int32
+ *     [n_faces before cleaning] of component numbers.  Outputs: component count, kept components, and the cleaned
+ *     mesh's n_verts / n_faces (each pointer may be NULL).  A context without a mesh holds the empty mesh.  Refuses a
+ *     mesh with max |coordinate| * n_verts >= 2^30 (int64 range of the sums) and leaves it resident unchanged. */
+int disn_mesh_load(disn_ctx* ctx, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces);
+int disn_mesh_clean(disn_ctx* ctx, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
+                    int64_t* n_kept, int64_t* n_verts, int64_t* n_faces);
 
 /* Estimated-camera path (reference: demo/demo.py:195-258 cam_evl, cam_est/model_cam.py:47-109, models/posenet.py:91-124):
  * imgs host [B,H,W,3] -> VGG-16 embedding (the context's `vgg_16/...` weights = the camera checkpoint's) -> three FC
