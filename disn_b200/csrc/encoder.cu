@@ -498,6 +498,10 @@ static const float* wptr(disn_ctx* c, const std::string& name) {
 }
 
 int encoder_gemv(disn_ctx* c, const float* x, const float* W, const float* bias, float* out, int B, int K, int N, int relu) {
+  // the partial sums live in c->partial, which exists only once the encoder buffers do: get_decoder runs without encode
+  if (encoder_alloc(c, 1)) return -1;
+  DISN_REQUIRE((int64_t)((K + GEMV_KS - 1) / GEMV_KS) * B * N <= (int64_t)((25088 + GEMV_KS - 1) / GEMV_KS) * c->alloc_B * 4096,
+               "gemv: partial sums exceed the encoder's buffer");
   return launch_gemv(c, x, W, bias, out, B, K, N, relu);
 }
 int encoder_gemm_plain(disn_ctx* c, const std::string& wname, const float* A, const float* Bm, const float* bias, float* C,

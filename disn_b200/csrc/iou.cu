@@ -9,8 +9,13 @@
 //   * a cell is occupied iff it overlaps at least one triangle (closed separating-axis test, 13 axes);
 //   * the voxel mesh's vertices are the 8 corners (k +- 1/2) * cell of every occupied cell.
 // The binning is the reference's expression; bins outside [0, dim) are dropped (numpy would wrap negatives and raise on
-// >= dim; ShapeNet meshes are normalised into the unit sphere so neither happens).  The CPU twin
-// oracle/metrics_oracle.py:iou_voxel does the same float64 operations in the same order; this file is compiled with
+// >= dim; ShapeNet meshes are normalised into the unit sphere so neither happens).
+// Voxel window: a corner p lands in a bin iff (p + 1.1) / 2.4 * dim is in (-1, dim), i.e. p in (-1.1 - 2.4/dim, 1.3), so
+// cell k can contribute only if k * cell is in (-1.1 - 2.4/dim - cell/2, 1.3 + cell/2) = (-(0.55 dim + 1.7), 0.65 dim + 0.5)
+// cells.  The hashed cells are k in [-voff, vhi) with voff = floor(11 dim / 20) + 4 and vhi = floor(13 dim / 20) + 4, which
+// covers that range with more than one cell to spare on each side (621^3 bits = 30 MB at dim 512); cells outside it
+// are skipped, which drops nothing.  The CPU twin oracle/metrics_oracle.py:iou_voxel derives the same window
+// (voxel_window) and does the same float64 operations in the same order; this file is compiled with
 // --fmad=false so that the classification is identical (tests assert equal occupancy grids).
 #include <algorithm>
 #include <cstring>
@@ -20,8 +25,18 @@
 namespace disn {
 namespace {
 
-constexpr int VG = 160;          // voxel index range [-80, 80) per axis: |coordinate| < 80 * 2/dim (1.45 for dim 110)
-constexpr int VOFF = 80;
+// voxel index range [-voff, vhi) per axis (see the window rule above)
+struct VoxWindow {
+  int voff, vhi, vg;
+};
+
+VoxWindow voxel_window(int dim) {
+  VoxWindow w;
+  w.voff = 11 * dim / 20 + 4;
+  w.vhi = 13 * dim / 20 + 4;
+  w.vg = w.voff + w.vhi;
+  return w;
+}
 
 __device__ __forceinline__ bool axis_sep(double ax, double ay, double az, const double v[3][3], double half) {
   const double p0 = ax * v[0][0] + ay * v[0][1] + az * v[0][2];
@@ -58,7 +73,8 @@ __device__ bool tri_cube_overlap(const double c[3], double half, const double t[
 }
 
 __global__ void voxelize_kernel(const float* __restrict__ verts, const int32_t* __restrict__ faces, int64_t nf, double cell,
-                                uint32_t* __restrict__ vox) {
+                                VoxWindow win, uint32_t* __restrict__ vox) {
+  const int64_t vg = win.vg;
   for (int64_t f = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; f < nf; f += (int64_t)gridDim.x * blockDim.x) {
     double t[3][3];
     double lo[3], hi[3];
@@ -70,30 +86,33 @@ __global__ void voxelize_kernel(const float* __restrict__ verts, const int32_t* 
     for (int a = 0; a < 3; ++a) {
       lo[a] = fmin(t[0][a], fmin(t[1][a], t[2][a]));
       hi[a] = fmax(t[0][a], fmax(t[1][a], t[2][a]));
-      k0[a] = max(-VOFF, (int)floor(lo[a] / cell - 0.5));
-      k1[a] = min(VOFF - 1, (int)ceil(hi[a] / cell + 0.5));
+      // clamped to the window in double before the cast, so that far-out coordinates cannot overflow it; a triangle
+      // entirely outside the window gets k1 < k0 on some axis and no cells
+      k0[a] = (int)fmin(fmax(floor(lo[a] / cell - 0.5), (double)-win.voff), (double)win.vhi);
+      k1[a] = (int)fmax(fmin(ceil(hi[a] / cell + 0.5), (double)(win.vhi - 1)), (double)(-win.voff - 1));
     }
     for (int kz = k0[2]; kz <= k1[2]; ++kz)
       for (int ky = k0[1]; ky <= k1[1]; ++ky)
         for (int kx = k0[0]; kx <= k1[0]; ++kx) {
           const double c[3] = {(double)kx * cell, (double)ky * cell, (double)kz * cell};
           if (!tri_cube_overlap(c, cell * 0.5, t)) continue;
-          const int64_t id = ((int64_t)(kz + VOFF) * VG + (ky + VOFF)) * VG + (kx + VOFF);
+          const int64_t id = ((int64_t)(kz + win.voff) * vg + (ky + win.voff)) * vg + (kx + win.voff);
           atomicOr(&vox[id >> 5], 1u << (id & 31));
         }
   }
 }
 
 // corners of occupied cells -> ((c + 1.1) / 2.4 * dim) truncated -> occupancy bits
-__global__ void corners_kernel(const uint32_t* __restrict__ vox, double cell, int dim, uint32_t* __restrict__ occ) {
-  const int64_t nwords = (int64_t)VG * VG * VG / 32;
+__global__ void corners_kernel(const uint32_t* __restrict__ vox, double cell, int dim, VoxWindow win,
+                               uint32_t* __restrict__ occ) {
+  const int64_t vg = win.vg, nwords = (vg * vg * vg + 31) / 32;
   for (int64_t w = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; w < nwords; w += (int64_t)gridDim.x * blockDim.x) {
     uint32_t bits = vox[w];
     while (bits) {
       const int b = __ffs(bits) - 1;
       bits &= bits - 1;
       const int64_t id = w * 32 + b;
-      const int kx = (int)(id % VG) - VOFF, ky = (int)((id / VG) % VG) - VOFF, kz = (int)(id / ((int64_t)VG * VG)) - VOFF;
+      const int kx = (int)(id % vg) - win.voff, ky = (int)((id / vg) % vg) - win.voff, kz = (int)(id / (vg * vg)) - win.voff;
       for (int cz = 0; cz < 2; ++cz)
         for (int cy = 0; cy < 2; ++cy)
           for (int cx = 0; cx < 2; ++cx) {
@@ -149,7 +168,8 @@ extern "C" int disn_iou(disn_ctx* c, const float* verts1, int64_t nv1, const int
     const int64_t nf = m ? nf2 : nf1, nv = m ? nv2 : nv1;
     for (int64_t i = 0; i < nf * 3; ++i) DISN_REQUIRE(f[i] >= 0 && f[i] < nv, "face index out of range");
   }
-  const int64_t vox_words = (int64_t)VG * VG * VG / 32, n_occ = (int64_t)dim * dim * dim, occ_words = (n_occ + 31) / 32;
+  const VoxWindow win = voxel_window(dim);
+  const int64_t vox_words = ((int64_t)win.vg * win.vg * win.vg + 31) / 32, n_occ = (int64_t)dim * dim * dim, occ_words = (n_occ + 31) / 32;
   const size_t bytes = (size_t)(nv1 + nv2) * 12 + (size_t)(nf1 + nf2) * 12 + (size_t)(vox_words + 2 * occ_words) * 4 + 16 +
                        (size_t)n_occ + 4096;
   char* base = nullptr;
@@ -176,8 +196,8 @@ extern "C" int disn_iou(disn_ctx* c, const float* verts1, int64_t nv1, const int
     if ((e = cudaMemcpyAsync(dv, hv, (size_t)nv * 12, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return fail("copy", e);
     if ((e = cudaMemcpyAsync(df, hf, (size_t)nf * 12, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) return fail("copy", e);
     if ((e = cudaMemsetAsync(vox, 0, vox_words * 4, c->stream)) != cudaSuccess) return fail("memset", e);
-    voxelize_kernel<<<grid, 128, 0, c->stream>>>(dv, df, nf, cell, vox);
-    corners_kernel<<<grid, 256, 0, c->stream>>>(vox, cell, dim, occ[m]);
+    voxelize_kernel<<<grid, 128, 0, c->stream>>>(dv, df, nf, cell, win, vox);
+    corners_kernel<<<grid, 256, 0, c->stream>>>(vox, cell, dim, win, occ[m]);
     c->launches += 2;
   }
   iou_count_kernel<<<grid, 256, 0, c->stream>>>(occ[0], occ[1], occ_words, cnt);

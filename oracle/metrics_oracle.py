@@ -161,7 +161,7 @@ def precision_recall_f(pred, src, thresholds):
 # loaded here): its voxeliser is restated -- cells k are cubes centred at k*cell with half-size cell/2 (PyMesh hash keys
 # are round(x / cell_size)), occupied iff they overlap a triangle (closed 13-axis separating-axis test), voxel-mesh
 # vertices = the 8 corners of every occupied cell.  The binning expression is the reference's.  PARITY UNPINNED vs PyMesh.
-# disn_b200/csrc/iou.cu performs the same float64 operations in the same order.
+# disn_b200/csrc/iou.cu performs the same float64 operations in the same order, over the same window of cells.
 # ----------------------------------------------------------------------------------------------------------------------
 def _tri_cube_overlap(c, half, tri):
     """c [M,3] cube centres, tri [3,3] -> bool [M]; closed separating-axis test, same operation order as iou.cu."""
@@ -191,16 +191,27 @@ def _tri_cube_overlap(c, half, tri):
     return ok
 
 
-def voxel_occupancy(verts, faces, dim=110, vg=160, voff=80):
-    """occupancy grid [dim,dim,dim] uint8 of one mesh (the `v1` of test/test_iou.py:215-217)."""
+def voxel_window(dim):
+    """(vg, voff): the cells k in [-voff, vg - voff) per axis that iou.cu hashes.  A corner p of a cell lands in a bin iff
+    (p + 1.1) / 2.4 * dim is in (-1, dim), so only cells with k * cell in (-1.1 - 2.4/dim - cell/2, 1.3 + cell/2), i.e.
+    k in (-(0.55 dim + 1.7), 0.65 dim + 0.5), can contribute; the window covers that with more than a cell to spare."""
+    voff, vhi = 11 * dim // 20 + 4, 13 * dim // 20 + 4
+    return voff + vhi, voff
+
+
+def voxel_occupancy(verts, faces, dim=110, vg=None, voff=None):
+    """occupancy grid [dim,dim,dim] uint8 of one mesh (the `v1` of test/test_iou.py:215-217).  Cells outside
+    [-voff, vg - voff) are skipped; by default the window of voxel_window(dim), which loses no occupied bin."""
+    if vg is None:
+        vg, voff = voxel_window(dim)
     cell = 2.0 / dim
     V = np.asarray(verts, np.float32).astype(np.float64)
     vox = set()
     for f in np.asarray(faces):
         tri = V[f]
         lo, hi = tri.min(axis=0), tri.max(axis=0)
-        k0 = np.maximum(-voff, np.floor(lo / cell - 0.5).astype(int))
-        k1 = np.minimum(voff - 1, np.ceil(hi / cell + 0.5).astype(int))
+        k0 = np.clip(np.floor(lo / cell - 0.5), -voff, vg - voff).astype(int)
+        k1 = np.clip(np.ceil(hi / cell + 0.5), -voff - 1, vg - voff - 1).astype(int)
         if np.any(k1 < k0):
             continue
         ks = np.stack(np.meshgrid(*[np.arange(k0[a], k1[a] + 1) for a in range(3)], indexing="ij"), axis=-1).reshape(-1, 3)
