@@ -6,6 +6,7 @@
 #include <map>
 #include <set>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/disn_b200.h"
@@ -32,10 +33,60 @@ void set_error(const std::string& msg);
     }                                                    \
   } while (0)
 
+// Sole owner of one device (cudaMalloc) or pinned host (cudaMallocHost) allocation: move-only, freed on destruction.
+template <bool Pinned>
+class Buffer {
+ public:
+  Buffer() = default;
+  Buffer(Buffer&& o) noexcept : p_(o.p_), bytes_(o.bytes_) { o.p_ = nullptr; o.bytes_ = 0; }
+  Buffer& operator=(Buffer&& o) noexcept { std::swap(p_, o.p_); std::swap(bytes_, o.bytes_); return *this; }
+  Buffer(const Buffer&) = delete;
+  Buffer& operator=(const Buffer&) = delete;
+  ~Buffer() { release(); }
+
+  // Grow only: when `need` exceeds the capacity, drops the old allocation (its contents are NOT kept) and allocates
+  // exactly need + slack bytes.  A failed allocation leaves the buffer empty and returns -1; the next call retries.
+  int ensure(size_t need, size_t slack = 0) {
+    if (need <= bytes_) return 0;
+    release();
+    void* p = nullptr;
+    DISN_CUDA_OK(Pinned ? cudaMallocHost(&p, need + slack) : cudaMalloc(&p, need + slack));
+    p_ = p;
+    bytes_ = need + slack;
+    return 0;
+  }
+  template <class T> T* as() const { return static_cast<T*>(p_); }
+  size_t bytes() const { return bytes_; }
+
+ private:
+  void release() {
+    if (p_) { if (Pinned) cudaFreeHost(p_); else cudaFree(p_); }
+    p_ = nullptr;
+    bytes_ = 0;
+  }
+  void* p_ = nullptr;
+  size_t bytes_ = 0;
+};
+using DevBuffer = Buffer<false>;
+using PinnedBuffer = Buffer<true>;
+
+// Carves 256-byte aligned pieces out of one allocation.  With a null base every take returns nullptr and only `off`
+// advances, so running the same takes first on nullptr sizes the allocation they are then carved from.
+struct Arena {
+  char* base;
+  size_t off = 0;
+  template <class T> T* take(size_t n) {
+    T* p = reinterpret_cast<T*>(base ? base + off : nullptr);
+    off += (n * sizeof(T) + 255) & ~(size_t)255;
+    return p;
+  }
+};
+
 struct DevTensor {
-  float* ptr = nullptr;
+  DevBuffer buf;
   std::vector<int64_t> shape;
   int64_t numel = 0;
+  float* ptr() const { return buf.as<float>(); }
 };
 
 // VGG-16 topology (reference spec: models/CNN/vgg.py:187-196)
@@ -90,7 +141,9 @@ constexpr int DISN_STATUS_FP16_OVERFLOW = 1;   // DISN_PREC_F16F8: an activation
 
 }  // namespace disn
 
+// Every allocation of the context is a buffer member: deleting the context frees them all.
 struct disn_ctx {
+  ~disn_ctx();                  // destroys the encoder graph and the stream if the context owns it (api.cu)
   disn_config cfg;
   cudaStream_t stream = nullptr;
   bool own_stream = true;
@@ -103,55 +156,51 @@ struct disn_ctx {
 
   // encoder state
   int32_t enc_B = 0;
-  int32_t alloc_B = 0;
-  float* img_in = nullptr;      // [B,H,W,3] as uploaded
-  float* img_rs = nullptr;      // [B,224,224,3]
-  float* act[2] = {nullptr, nullptr};   // ping-pong activations
-  float* taps[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  float* proj[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // per-level projected maps [B,h,h,512]
-  float* fc_a = nullptr;        // [B,4096]
-  float* fc_b = nullptr;        // [B,4096]
-  float* partial = nullptr;     // split-K partials (fc layers)
-  float* splitk_ws = nullptr;   // split-K partials (conv / projection GEMMs)
-  int64_t splitk_ws_elems = 0;
-  float* emb = nullptr;         // [B,num_classes]
-  float* gbias = nullptr;       // [B,512]
-  float* pmap = nullptr;        // [B,img_h,img_w,512]
+  int32_t alloc_B = 0;          // batch the encoder buffers are sized for
+  disn::DevBuffer img_in;       // [B,H,W,3] as uploaded
+  disn::DevBuffer img_rs;       // [B,224,224,3]
+  disn::DevBuffer act[2];       // ping-pong activations
+  disn::DevBuffer taps[5];
+  disn::DevBuffer proj[5];      // per-level projected maps [B,h,h,512]
+  disn::DevBuffer fc_a;         // [B,4096]
+  disn::DevBuffer fc_b;         // [B,4096]
+  disn::DevBuffer partial;      // split-K partials (fc layers)
+  disn::DevBuffer splitk_ws;    // split-K partials (conv / projection GEMMs)
+  disn::DevBuffer emb;          // [B,num_classes]
+  disn::DevBuffer gbias;        // [B,512]
+  disn::DevBuffer pmap;         // [B,img_h,img_w,512]
   cudaGraphExec_t enc_graph_exec = nullptr;   // captured encoder launch sequence (encoder_run)
   std::vector<int64_t> enc_graph_key, enc_warm_key;
   int64_t enc_graph_launches = 0;
   // scratch for host-pointer calls
-  float* d_pts = nullptr; float* d_pts_rot = nullptr; float* d_out = nullptr; float* d_uv = nullptr;
-  int64_t scratch_pts = 0;
-  float* d_tm = nullptr;        // [max_batch,4,3]
-  int* d_status = nullptr;      // device status word (PointJob::status)
-  int* h_status = nullptr;      // pinned host mirror, copied behind every point-kernel launch
-  float* d_axes = nullptr;      // [max_batch,3,R]
-  int32_t axes_R = 0;
+  disn::DevBuffer d_pts, d_pts_rot, d_out, d_uv;
+  disn::DevBuffer d_tm;         // [max_batch,4,3]
+  disn::DevBuffer d_status;     // device status word (PointJob::status)
+  disn::PinnedBuffer h_status;  // pinned host mirror, copied behind every point-kernel launch
+  disn::DevBuffer d_axes;       // [max_batch,3,R]
   std::vector<double> axes_key; // (sdf_params, R) the tables in d_axes were built from
   // bf16x3 packed weights (tensor-core path)
-  void* tc_weights = nullptr;          // bf16 hi/lo stage images of the point MLP (DISN_PREC_BF16X3)
-  int64_t tc_weights_bytes = 0;
-  void* tc_weights_f8 = nullptr;       // fp16 + e5m2 stage images (DISN_PREC_F16F8)
+  disn::DevBuffer tc_weights;          // bf16 hi/lo stage images of the point MLP (DISN_PREC_BF16X3)
+  disn::DevBuffer tc_weights_f8;       // fp16 + e5m2 stage images (DISN_PREC_F16F8)
   float tc_act_scale[2][4][2] = {};
   float tc_small[2][2048] = {};         // host copy of the per-stream small parameters (the point kernel's __grid_constant__ table)
-  std::map<std::string, uint8_t*> enc_tc_weights;   // packed bf16 hi/lo stage images of the encoder GEMMs
+  std::map<std::string, disn::DevBuffer> enc_tc_weights;   // packed bf16 hi/lo stage images of the encoder GEMMs
   // marching cubes: persistent scratch + the device-resident mesh of the last run (mc.cu)
-  uint8_t* mc_code = nullptr; uint32_t* mc_vbase = nullptr; uint32_t* mc_chunk = nullptr; uint32_t* mc_sums = nullptr;
-  uint32_t* mc_totals = nullptr; uint32_t* mc_totals_host = nullptr;
-  float* mc_verts = nullptr; int32_t* mc_faces = nullptr;
-  int64_t mc_pts_cap = 0, mc_verts_cap = 0, mc_faces_cap = 0, mc_nv = 0, mc_nf = 0;
+  disn::DevBuffer mc_code, mc_vbase, mc_chunk, mc_sums, mc_totals;
+  disn::PinnedBuffer mc_totals_host;
+  disn::DevBuffer mc_verts, mc_faces;
+  int64_t mc_nv = 0, mc_nf = 0;
   // small-part cleaning of the resident mesh (mesh_clean.cu): scratch arena, the compacted mesh's buffers (swapped with
   // mc_verts / mc_faces after a clean) and the totals read back once per clean; all grow only
-  void* cl_arena = nullptr; int64_t cl_arena_bytes = 0;
-  float* cl_verts = nullptr; int32_t* cl_faces = nullptr; int64_t cl_verts_cap = 0, cl_faces_cap = 0;
-  uint32_t* cl_totals_host = nullptr;
+  disn::DevBuffer cl_arena;
+  disn::DevBuffer cl_verts, cl_faces;
+  disn::PinnedBuffer cl_totals_host;
   // device-resident SDF grid of disn_eval_grid_resident and host staging for the marching-cubes input
-  float* d_grid = nullptr; int64_t grid_cap = 0;
-  float* d_mc_in = nullptr; int64_t mc_in_cap = 0;
+  disn::DevBuffer d_grid;
+  disn::DevBuffer d_mc_in;
   // nn_distance / cam scratch (persistent, grows)
-  void* nn_scratch = nullptr; int64_t nn_scratch_bytes = 0;
-  void* dec_scratch = nullptr; int64_t dec_scratch_bytes = 0;   // explicit-feature decoder staging (decoder.cu)
+  disn::DevBuffer nn_scratch;
+  disn::DevBuffer dec_scratch;  // explicit-feature decoder staging (decoder.cu)
 };
 
 namespace disn {
@@ -159,7 +208,6 @@ namespace disn {
 int encoder_alloc(disn_ctx* c, int B);
 int encoder_run(disn_ctx* c, const float* imgs, int B, int H, int W, int C, bool device_ptr,
                 bool embedding_only = false);
-void encoder_free(disn_ctx* c);
 void encoder_graph_reset(disn_ctx* c);
 // api.cu
 int run_point_job(disn_ctx* c, PointJob& job);    // fills weights / encoder products / status and launches per cfg.precision
@@ -174,7 +222,7 @@ int launch_point_fp32(disn_ctx* c, const PointJob& job);
 int tc_pack_weights(disn_ctx* c);
 int launch_point_tc(disn_ctx* c, const PointJob& job);
 // conv_tc.cu
-int conv_tc_pack(disn_ctx* c, const float* d_w, int K, int N, uint8_t** out_dev);
+int conv_tc_pack(disn_ctx* c, const float* d_w, int K, int N, DevBuffer& out);
 int launch_conv_tc(disn_ctx* c, const float* A, const uint8_t* wpk, const float* bias, float* C, float* ws,
                    int64_t ws_elems, int M, int N, int K, int H, int W, int Cin, int relu, int* splits_out);
 // cam.cu
@@ -185,7 +233,8 @@ int nn_distance(disn_ctx* c, const float* d_xyz1, int n, const float* d_xyz2, in
 // mc.cu
 int mc_run(disn_ctx* c, const float* d_sdf, int R, const double* bbox, float iso, int64_t* n_verts, int64_t* n_faces);
 int mc_fetch(disn_ctx* c, float* verts, int32_t* faces);
-void mc_free(disn_ctx* c);
+// grow-only vertex [nv,3] and face [nf,3] arrays of a mesh, with 25 % + 1024 elements of slack
+int ensure_mesh(DevBuffer& verts, DevBuffer& faces, int64_t nv, int64_t nf);
 // in-place exclusive scan of d[0..n) on c->stream, total -> *d_total (device); `sums` = scan_scratch_elems(n) words
 int64_t scan_scratch_elems(int64_t n);
 int exclusive_scan(disn_ctx* c, uint32_t* d, int64_t n, uint32_t* d_total, uint32_t* sums);
@@ -193,5 +242,4 @@ int exclusive_scan(disn_ctx* c, uint32_t* d, int64_t n, uint32_t* d_total, uint3
 int mesh_load(disn_ctx* c, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces);
 int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
                int64_t* n_kept, int64_t* n_verts, int64_t* n_faces);
-void mesh_clean_free(disn_ctx* c);
 }  // namespace disn

@@ -182,7 +182,7 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(ConvTcJob job) {
 }  // namespace
 
 // [K, N] fp32 row-major (device) -> packed B stage images [N/128][K/64][hi|lo][128 x 64 SW128 bf16] (device)
-int conv_tc_pack(disn_ctx* c, const float* d_w, int K, int N, uint8_t** out_dev) {
+int conv_tc_pack(disn_ctx* c, const float* d_w, int K, int N, DevBuffer& out) {
   std::vector<float> w((size_t)K * N);
   DISN_CUDA_OK(cudaMemcpyAsync(w.data(), d_w, w.size() * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
@@ -202,8 +202,8 @@ int conv_tc_pack(disn_ctx* c, const float* d_w, int K, int N, uint8_t** out_dev)
       }
   // copy on the context's (non-blocking) stream and wait: a plain cudaMemcpy from pageable memory may return before
   // the DMA has landed and is not ordered against kernels on a non-blocking stream
-  DISN_CUDA_OK(cudaMalloc(out_dev, img.size()));
-  DISN_CUDA_OK(cudaMemcpyAsync(*out_dev, img.data(), img.size(), cudaMemcpyHostToDevice, c->stream));
+  if (out.ensure(img.size())) return -1;
+  DISN_CUDA_OK(cudaMemcpyAsync(out.as<uint8_t>(), img.data(), img.size(), cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
   return 0;
 }

@@ -147,17 +147,6 @@ __global__ void __launch_bounds__(EM_THREADS) match_cost_sum_kernel(const double
   if (threadIdx.x == 0) cost[b] = __double2float_rn(part[0]);
 }
 
-struct DevBuf {       // one allocation, released on every exit path
-  char* base = nullptr;
-  char* p = nullptr;
-  ~DevBuf() { if (base) cudaFree(base); }
-  template <class T> T* take(size_t count) {
-    T* r = reinterpret_cast<T*>(p);
-    p += (count * sizeof(T) + 255) / 256 * 256;
-    return r;
-  }
-};
-
 int match_cost_device(disn_ctx* c, const float* d1, const float* d2, const float* dmatch, int B, int N, int M, double* rowcost,
                       float* dcost) {
   match_cost_rows_kernel<<<dim3((N + EM_WARPS - 1) / EM_WARPS, B), EM_THREADS, 0, c->stream>>>(d1, d2, dmatch, N, M, rowcost);
@@ -178,19 +167,24 @@ extern "C" int disn_approx_match(disn_ctx* c, const float* xyz1, const float* xy
   DISN_REQUIRE(B >= 1 && N >= 1 && M >= 1 && B <= 65535, "ApproxMatch expects (batch_size,num_points,3) point sets, batch <= 65535");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
   const size_t n1 = (size_t)B * N, n2 = (size_t)B * M, nm = (size_t)B * N * M;
-  DevBuf buf;
-  const size_t bytes = (n1 + n2) * 12 + (3 * n1 + 3 * n2) * 8 + nm * 4 + n1 * 8 + (size_t)B * 4 + 16 * 256;
-  DISN_CUDA_OK(cudaMalloc(&buf.base, bytes));
-  buf.p = buf.base;
-  float* d1 = buf.take<float>(n1 * 3);
-  float* d2 = buf.take<float>(n2 * 3);
-  double* satl[2] = {buf.take<double>(n1), buf.take<double>(n1)};
-  double* satr[2] = {buf.take<double>(n2), buf.take<double>(n2)};
-  double* s = buf.take<double>(n1);
-  double* clip = buf.take<double>(n2);
-  float* dmatch = buf.take<float>(nm);
-  double* rowcost = buf.take<double>(n1);
-  float* dcost = buf.take<float>(B);
+  float *d1, *d2, *dmatch, *dcost;
+  double *satl[2], *satr[2], *s, *clip, *rowcost;
+  auto carve = [&](char* base) {
+    Arena a{base};
+    d1 = a.take<float>(n1 * 3);
+    d2 = a.take<float>(n2 * 3);
+    satl[0] = a.take<double>(n1); satl[1] = a.take<double>(n1);
+    satr[0] = a.take<double>(n2); satr[1] = a.take<double>(n2);
+    s = a.take<double>(n1);
+    clip = a.take<double>(n2);
+    dmatch = a.take<float>(nm);
+    rowcost = a.take<double>(n1);
+    dcost = a.take<float>(B);
+    return a.off;
+  };
+  DevBuffer buf;     // per call, freed on every exit path
+  if (buf.ensure(carve(nullptr))) return -1;
+  carve(buf.as<char>());
   DISN_CUDA_OK(cudaMemcpyAsync(d1, xyz1, n1 * 12, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaMemcpyAsync(d2, xyz2, n2 * 12, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaMemsetAsync(dmatch, 0, nm * 4, c->stream));
@@ -228,14 +222,20 @@ extern "C" int disn_match_cost(disn_ctx* c, const float* xyz1, const float* xyz2
   DISN_REQUIRE(B >= 1 && N >= 1 && M >= 1 && B <= 65535, "MatchCost expects (batch_size,num_points,3) point sets, batch <= 65535");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
   const size_t n1 = (size_t)B * N, n2 = (size_t)B * M, nm = (size_t)B * N * M;
-  DevBuf buf;
-  DISN_CUDA_OK(cudaMalloc(&buf.base, (n1 + n2) * 12 + nm * 4 + n1 * 8 + (size_t)B * 4 + 8 * 256));
-  buf.p = buf.base;
-  float* d1 = buf.take<float>(n1 * 3);
-  float* d2 = buf.take<float>(n2 * 3);
-  float* dmatch = buf.take<float>(nm);
-  double* rowcost = buf.take<double>(n1);
-  float* dcost = buf.take<float>(B);
+  float *d1, *d2, *dmatch, *dcost;
+  double* rowcost;
+  auto carve = [&](char* base) {
+    Arena a{base};
+    d1 = a.take<float>(n1 * 3);
+    d2 = a.take<float>(n2 * 3);
+    dmatch = a.take<float>(nm);
+    rowcost = a.take<double>(n1);
+    dcost = a.take<float>(B);
+    return a.off;
+  };
+  DevBuffer buf;     // per call, freed on every exit path
+  if (buf.ensure(carve(nullptr))) return -1;
+  carve(buf.as<char>());
   DISN_CUDA_OK(cudaMemcpyAsync(d1, xyz1, n1 * 12, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaMemcpyAsync(d2, xyz2, n2 * 12, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaMemcpyAsync(dmatch, match, nm * 4, cudaMemcpyHostToDevice, c->stream));

@@ -249,17 +249,6 @@ __global__ void __launch_bounds__(CL_THREADS) clean_compact_faces_kernel(const i
   for (int j = 0; j < 3; ++j) out[3 * (int64_t)o + j] = (int32_t)vmap[faces[3 * f + j]];
 }
 
-// carve the arena into 256-byte aligned pieces
-struct Arena {
-  char* base;
-  int64_t off = 0;
-  template <class T> T* take(int64_t n) {
-    T* p = reinterpret_cast<T*>(base ? base + off : nullptr);
-    off += (n * (int64_t)sizeof(T) + 255) & ~(int64_t)255;
-    return p;
-  }
-};
-
 struct CleanBufs {
   uint32_t *offs, *cursor, *vflag, *rflag, *fflag, *cnt, *scan, *totals;
   int32_t *inc, *label;
@@ -267,7 +256,7 @@ struct CleanBufs {
   uint8_t* keep;
 };
 
-int64_t carve(char* base, int64_t nv, int64_t nf, CleanBufs& b) {
+size_t carve(char* base, int64_t nv, int64_t nf, CleanBufs& b) {
   Arena a{base};
   b.offs = a.take<uint32_t>(nv + 1);
   b.cursor = a.take<uint32_t>(nv);
@@ -284,25 +273,7 @@ int64_t carve(char* base, int64_t nv, int64_t nf, CleanBufs& b) {
   return a.off;
 }
 
-int grow(disn_ctx* c, void** p, int64_t* cap, int64_t n, size_t elem) {
-  if (n <= *cap) return 0;
-  if (*p) cudaFree(*p);
-  *p = nullptr; *cap = 0;
-  const int64_t want = n + n / 4 + 1024;
-  DISN_CUDA_OK(cudaMalloc(p, (size_t)want * elem));
-  *cap = want;
-  return 0;
-}
-
 }  // namespace
-
-void mesh_clean_free(disn_ctx* c) {
-  for (void* p : {c->cl_arena, (void*)c->cl_verts, (void*)c->cl_faces})
-    if (p) cudaFree(p);
-  if (c->cl_totals_host) cudaFreeHost(c->cl_totals_host);
-  c->cl_arena = nullptr; c->cl_verts = nullptr; c->cl_faces = nullptr; c->cl_totals_host = nullptr;
-  c->cl_arena_bytes = c->cl_verts_cap = c->cl_faces_cap = 0;
-}
 
 // Upload a host mesh into the resident mesh slot marching cubes fills (verts [nv,3] float32, faces [nf,3] int32 0-based).
 int mesh_load(disn_ctx* c, const float* verts, int64_t nv, const int32_t* faces, int64_t nf) {
@@ -312,10 +283,13 @@ int mesh_load(disn_ctx* c, const float* verts, int64_t nv, const int32_t* faces,
     if (faces[i] < 0 || faces[i] >= nv)
       DISN_REQUIRE(false, "face " + std::to_string(i / 3) + " references vertex " + std::to_string(faces[i]) +
                               " outside [0, " + std::to_string(nv) + ")");
-  if (grow(c, (void**)&c->mc_verts, &c->mc_verts_cap, nv, 3 * sizeof(float))) return -1;
-  if (grow(c, (void**)&c->mc_faces, &c->mc_faces_cap, nf, 3 * sizeof(int32_t))) return -1;
-  if (nv) DISN_CUDA_OK(cudaMemcpyAsync(c->mc_verts, verts, (size_t)nv * 3 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  if (nf) DISN_CUDA_OK(cudaMemcpyAsync(c->mc_faces, faces, (size_t)nf * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  if (ensure_mesh(c->mc_verts, c->mc_faces, nv, nf)) return -1;
+  if (nv)
+    DISN_CUDA_OK(cudaMemcpyAsync(c->mc_verts.as<float>(), verts, (size_t)nv * 3 * sizeof(float), cudaMemcpyHostToDevice,
+                                 c->stream));
+  if (nf)
+    DISN_CUDA_OK(cudaMemcpyAsync(c->mc_faces.as<int32_t>(), faces, (size_t)nf * 3 * sizeof(int32_t),
+                                 cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
   c->mc_nv = nv; c->mc_nf = nf;
   return 0;
@@ -342,21 +316,15 @@ int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face
     return 0;
   }
   CleanBufs b;
-  const int64_t bytes = carve(nullptr, nv, nf, b);
-  if (bytes > c->cl_arena_bytes) {
-    if (c->cl_arena) cudaFree(c->cl_arena);
-    c->cl_arena = nullptr; c->cl_arena_bytes = 0;
-    DISN_CUDA_OK(cudaMalloc(&c->cl_arena, (size_t)(bytes + bytes / 4)));
-    c->cl_arena_bytes = bytes + bytes / 4;
-  }
-  carve((char*)c->cl_arena, nv, nf, b);
-  if (!c->cl_totals_host) DISN_CUDA_OK(cudaMallocHost(&c->cl_totals_host, T_COUNT * sizeof(uint32_t)));
-  if (grow(c, (void**)&c->cl_verts, &c->cl_verts_cap, nv, 3 * sizeof(float))) return -1;
-  if (grow(c, (void**)&c->cl_faces, &c->cl_faces_cap, nf, 3 * sizeof(int32_t))) return -1;
+  const size_t bytes = carve(nullptr, nv, nf, b);
+  if (c->cl_arena.ensure(bytes, bytes / 4) || c->cl_totals_host.ensure(T_COUNT * sizeof(uint32_t)) ||
+      ensure_mesh(c->cl_verts, c->cl_faces, nv, nf))
+    return -1;
+  carve(c->cl_arena.as<char>(), nv, nf, b);
 
   cudaStream_t s = c->stream;
-  const float* verts = c->mc_verts;
-  const int32_t* faces = c->mc_faces;
+  const float* verts = c->mc_verts.as<float>();
+  const int32_t* faces = c->mc_faces.as<int32_t>();
   uint32_t* T = b.totals;
   DISN_CUDA_OK(cudaMemsetAsync(b.offs, 0, (size_t)(nv + 1) * sizeof(uint32_t), s));
   DISN_CUDA_OK(cudaMemsetAsync(b.vflag, 0, (size_t)(nv + 1) * sizeof(uint32_t), s));
@@ -384,24 +352,24 @@ int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face
   DISN_CUDA_OK(cudaGetLastError());
   if (exclusive_scan(c, b.fflag, nf + 1, T + T_NF_OUT, b.scan)) return -1;
   if (exclusive_scan(c, b.vflag, nv + 1, T + T_NV_OUT, b.scan)) return -1;
-  clean_compact_verts_kernel<<<grid_of(nv), CL_THREADS, 0, s>>>(verts, nv, b.vflag, c->cl_verts);
-  clean_compact_faces_kernel<<<grid_of(nf), CL_THREADS, 0, s>>>(faces, nf, b.fflag, b.vflag, c->cl_faces);
+  clean_compact_verts_kernel<<<grid_of(nv), CL_THREADS, 0, s>>>(verts, nv, b.vflag, c->cl_verts.as<float>());
+  clean_compact_faces_kernel<<<grid_of(nf), CL_THREADS, 0, s>>>(faces, nf, b.fflag, b.vflag, c->cl_faces.as<int32_t>());
   c->launches += 2;
   DISN_CUDA_OK(cudaGetLastError());
   if (face_component)
     DISN_CUDA_OK(cudaMemcpyAsync(face_component, b.label, (size_t)nf * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  DISN_CUDA_OK(cudaMemcpyAsync(c->cl_totals_host, T, T_COUNT * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  uint32_t* h = c->cl_totals_host.as<uint32_t>();
+  DISN_CUDA_OK(cudaMemcpyAsync(h, T, T_COUNT * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   DISN_CUDA_OK(cudaStreamSynchronize(s));
 
-  const uint32_t* h = c->cl_totals_host;
   float maxabs_f;
   std::memcpy(&maxabs_f, &h[T_MAXABS], sizeof(float));
   const double maxabs = (double)maxabs_f;
   DISN_REQUIRE(maxabs * (double)nv < 1073741824.0,
                "mesh_clean: max |coordinate| * n_verts = " + std::to_string(maxabs * (double)nv) +
                    " must stay below 2^30 (int64 fixed-point centroid sums)");
-  std::swap(c->mc_verts, c->cl_verts); std::swap(c->mc_verts_cap, c->cl_verts_cap);
-  std::swap(c->mc_faces, c->cl_faces); std::swap(c->mc_faces_cap, c->cl_faces_cap);
+  std::swap(c->mc_verts, c->cl_verts);
+  std::swap(c->mc_faces, c->cl_faces);
   c->mc_nv = h[T_NV_OUT];
   c->mc_nf = h[T_NF_OUT];
   out(h[T_NCOMP], h[T_NKEPT]);

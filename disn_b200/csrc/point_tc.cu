@@ -436,7 +436,8 @@ int tc_pack_weights(disn_ctx* c) {
       DISN_REQUIRE(it != c->weights.end(), "missing variable " + p + names[layer]);
       const int K = layer_k(layer), N = layer_n(layer);
       std::vector<float> w((size_t)K * N);   // rows 0..K-1 of the [Cin,Cout] matrix (point-feature part)
-      DISN_CUDA_OK(cudaMemcpyAsync(w.data(), it->second.ptr, w.size() * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+      DISN_CUDA_OK(cudaMemcpyAsync(w.data(), it->second.ptr(), w.size() * sizeof(float), cudaMemcpyDeviceToHost,
+                                   c->stream));
       DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
       for (int t = 0; t < K / 64; ++t)
         for (int nb = 0; nb < N / 256; ++nb, ++stage)
@@ -457,15 +458,8 @@ int tc_pack_weights(disn_ctx* c) {
     }
   }
   DISN_REQUIRE(stage == (size_t)2 * STAGES_PER_STREAM, "internal: stage count");
-  if (c->tc_weights_bytes != (int64_t)total) {
-    if (c->tc_weights) cudaFree(c->tc_weights);
-    if (c->tc_weights_f8) cudaFree(c->tc_weights_f8);
-    c->tc_weights = c->tc_weights_f8 = nullptr;
-    DISN_CUDA_OK(cudaMalloc(&c->tc_weights, total));
-    DISN_CUDA_OK(cudaMalloc(&c->tc_weights_f8, total));
-    c->tc_weights_bytes = (int64_t)total;
-  }
-  DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights, img.data(), total, cudaMemcpyHostToDevice, c->stream));
+  if (c->tc_weights.ensure(total) || c->tc_weights_f8.ensure(total)) return -1;
+  DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights.as<void>(), img.data(), total, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));   // ordered on the ctx stream (see conv_tc_pack)
 
   // ---- DISN_PREC_F16F8 images: per half-stage: [fp16 W, SW128, 16 KB | e5m2(w.2^-s1), SW64, 8 KB |
@@ -480,7 +474,8 @@ int tc_pack_weights(disn_ctx* c) {
       auto it = c->weights.find(p + names[layer]);
       const int K = layer_k(layer), N = layer_n(layer);
       std::vector<float> w((size_t)K * N);
-      DISN_CUDA_OK(cudaMemcpyAsync(w.data(), it->second.ptr, w.size() * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+      DISN_CUDA_OK(cudaMemcpyAsync(w.data(), it->second.ptr(), w.size() * sizeof(float), cudaMemcpyDeviceToHost,
+                                   c->stream));
       DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
       double ss = 0;
       for (float v : w) ss += (double)v * v;
@@ -509,7 +504,7 @@ int tc_pack_weights(disn_ctx* c) {
           }
     }
   }
-  DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights_f8, img.data(), total, cudaMemcpyHostToDevice, c->stream));
+  DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights_f8.as<void>(), img.data(), total, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
 
   // host copy of the small per-stream parameters at the SB_* offsets (the kernel's __grid_constant__ parameter table)
@@ -522,7 +517,7 @@ int tc_pack_weights(disn_ctx* c) {
     for (const auto& e : small) {
       auto it = c->weights.find(p + e.name);
       DISN_REQUIRE(it != c->weights.end() && it->second.numel == e.n, "missing or mis-shaped variable " + p + e.name);
-      DISN_CUDA_OK(cudaMemcpyAsync(&c->tc_small[sidx][e.off], it->second.ptr, (size_t)e.n * sizeof(float),
+      DISN_CUDA_OK(cudaMemcpyAsync(&c->tc_small[sidx][e.off], it->second.ptr(), (size_t)e.n * sizeof(float),
                                    cudaMemcpyDeviceToHost, c->stream));
     }
   }
@@ -532,7 +527,7 @@ int tc_pack_weights(disn_ctx* c) {
 
 int launch_point_tc(disn_ctx* c, const PointJob& job_in) {
   const bool f8 = c->cfg.precision == DISN_PREC_F16F8;
-  const void* wpk = f8 ? c->tc_weights_f8 : c->tc_weights;
+  const void* wpk = (f8 ? c->tc_weights_f8 : c->tc_weights).as<void>();
   DISN_REQUIRE(wpk != nullptr, "tensor-core weights not packed (call disn_finalize_weights)");
   static_assert(sizeof(SmallParams) == sizeof(c->tc_small), "small-parameter table layout");
   PointJob job = job_in;
