@@ -59,6 +59,9 @@ EXPORTS = {
     "disn_mesh_load": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]),
     "disn_mesh_clean": (C.c_int, [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.POINTER(C.c_int64),
                                   C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "disn_mesh_sdf": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_double, C.c_double, C.c_void_p,
+                                C.POINTER(C.c_double), C.c_uint32]),
+    "disn_mesh_sdf_phase_ms": (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
     "disn_fetch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]),
     "disn_shared_alloc": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_void_p), C.c_char_p]),
     "disn_shared_open": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

@@ -16,6 +16,8 @@ using namespace disn;
 
 disn_ctx::~disn_ctx() {
   encoder_graph_reset(this);
+  for (cudaEvent_t e : sdf_ev)
+    if (e) cudaEventDestroy(e);
   if (own_stream && stream) cudaStreamDestroy(stream);
 }
 
@@ -512,6 +514,28 @@ int disn_mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t*
   return mesh_clean(c, dist_thresh, num_thresh, face_component, n_components, n_kept, n_verts, n_faces);
 }
 
+int disn_mesh_sdf(disn_ctx* c, int32_t res, const double* bbox, double expand_rate, double sigma, float* out,
+                  double* bbox_out, uint32_t flags) {
+  DISN_REQUIRE(c && out, "null argument");
+  DISN_REQUIRE(res >= 1, "mesh_sdf: res >= 1");
+  DISN_REQUIRE((int64_t)(res + 1) * (res + 1) * (res + 1) <= INT32_MAX,
+               "mesh_sdf: (res+1)^3 grid points must fit a 32-bit index (res <= 1289)");
+  DISN_REQUIRE(std::isfinite(sigma) && sigma >= 0.0, "mesh_sdf: sigma must be finite and >= 0");
+  DISN_REQUIRE(bbox || (std::isfinite(expand_rate) && expand_rate > 0.0), "mesh_sdf: expand_rate must be finite and > 0");
+  if (bbox)
+    for (int a = 0; a < 3; ++a)
+      DISN_REQUIRE(std::isfinite(bbox[a]) && std::isfinite(bbox[3 + a]) && bbox[a] < bbox[3 + a],
+                   "mesh_sdf: box min must be below max on every axis");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  return mesh_sdf(c, res, bbox, expand_rate, sigma, out, bbox_out, (flags & DISN_DEVICE_PTR) != 0);
+}
+
+int disn_mesh_sdf_phase_ms(disn_ctx* c, float* ms) {
+  DISN_REQUIRE(c && ms, "null argument");
+  for (int i = 0; i < 4; ++i) ms[i] = c->sdf_phase_ms[i];
+  return 0;
+}
+
 int disn_eval_grid_resident(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t B, int32_t sdf_res,
                             float** out_dev) {
   DISN_REQUIRE(c && sdf_params && trans_mat && out_dev, "null argument");
@@ -572,3 +596,5 @@ int disn_fetch(disn_ctx* c, const void* dev, void* host, int64_t bytes) {
 }
 
 }  // extern "C"
+
+void disn::axis_table(double start, double stop, int num, float* out) { linspace_f32(start, stop, num, out); }

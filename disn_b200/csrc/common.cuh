@@ -82,6 +82,47 @@ struct Arena {
   }
 };
 
+// Lock-free union-find over an int32 parent array (mesh_clean.cu: faces; mesh_sdf.cu: grid points).
+// Root of x with intermediate pointer jumping.  parent[x] <= x always holds (a root is only ever hooked under a smaller
+// root), so the root of a component is its smallest face.  Concurrent jumps only replace a pointer by an ancestor.
+__device__ __forceinline__ int32_t uf_find(volatile int32_t* parent, int32_t x) {
+  int32_t cur = parent[x];
+  if (cur != x) {
+    int32_t prev = x, next;
+    while (cur > (next = parent[cur])) {
+      parent[prev] = next;
+      prev = cur;
+      cur = next;
+    }
+  }
+  return cur;
+}
+
+// hook the larger root under the smaller one; a failed CAS means the root moved: continue from its new parent
+__device__ __forceinline__ void uf_union(int32_t* parent, int32_t a, int32_t b) {
+  int32_t ra = uf_find(parent, a), rb = uf_find(parent, b);
+  while (ra != rb) {
+    if (ra < rb) {
+      const int32_t old = atomicCAS(&parent[rb], rb, ra);
+      if (old == rb) break;
+      rb = old;
+    } else {
+      const int32_t old = atomicCAS(&parent[ra], ra, rb);
+      if (old == ra) break;
+      ra = old;
+    }
+  }
+}
+
+// Root of x by a read-only walk (for the flattening pass: a pointer-jumping store from another thread could otherwise
+// overwrite the root this thread stored).
+__device__ __forceinline__ int32_t uf_root(const int32_t* parent, int32_t x) {
+  volatile const int32_t* p = parent;
+  int32_t n;
+  while ((n = p[x]) != x) x = n;
+  return x;
+}
+
 struct DevTensor {
   DevBuffer buf;
   std::vector<int64_t> shape;
@@ -195,6 +236,12 @@ struct disn_ctx {
   disn::DevBuffer cl_arena;
   disn::DevBuffer cl_verts, cl_faces;
   disn::PinnedBuffer cl_totals_host;
+  // signed distance field of the resident mesh (mesh_sdf.cu): scratch arena (BVH, edge bits, union-find parents, the
+  // distance grid of host-output calls), pinned staging (mesh statistics, axis tables) and the phase timing events
+  disn::DevBuffer sdf_arena;
+  disn::PinnedBuffer sdf_host;
+  cudaEvent_t sdf_ev[5] = {};
+  float sdf_phase_ms[4] = {};
   // device-resident SDF grid of disn_eval_grid_resident and host staging for the marching-cubes input
   disn::DevBuffer d_grid;
   disn::DevBuffer d_mc_in;
@@ -242,4 +289,9 @@ int exclusive_scan(disn_ctx* c, uint32_t* d, int64_t n, uint32_t* d_total, uint3
 int mesh_load(disn_ctx* c, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces);
 int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
                int64_t* n_kept, int64_t* n_verts, int64_t* n_faces);
+// mesh_sdf.cu
+int mesh_sdf(disn_ctx* c, int32_t res, const double* bbox, double expand_rate, double sigma, float* out,
+             double* bbox_out, bool device_out);
+// api.cu: numpy.linspace(start, stop, num) in float64 cast to float32 (the grid coordinates of eval_grid and mesh_sdf)
+void axis_table(double start, double stop, int num, float* out);
 }  // namespace disn

@@ -45,37 +45,6 @@ __global__ void __launch_bounds__(CL_THREADS) clean_scatter_kernel(const int32_t
   for (int k = 0; k < 3; ++k) inc[atomicAdd(&cursor[faces[3 * f + k]], 1u)] = (int32_t)f;
 }
 
-// Root of x with intermediate pointer jumping.  parent[x] <= x always holds (a root is only ever hooked under a smaller
-// root), so the root of a component is its smallest face.  Concurrent jumps only replace a pointer by an ancestor.
-__device__ __forceinline__ int32_t uf_find(volatile int32_t* parent, int32_t x) {
-  int32_t cur = parent[x];
-  if (cur != x) {
-    int32_t prev = x, next;
-    while (cur > (next = parent[cur])) {
-      parent[prev] = next;
-      prev = cur;
-      cur = next;
-    }
-  }
-  return cur;
-}
-
-// hook the larger root under the smaller one; a failed CAS means the root moved: continue from its new parent
-__device__ __forceinline__ void uf_union(int32_t* parent, int32_t a, int32_t b) {
-  int32_t ra = uf_find(parent, a), rb = uf_find(parent, b);
-  while (ra != rb) {
-    if (ra < rb) {
-      const int32_t old = atomicCAS(&parent[rb], rb, ra);
-      if (old == rb) break;
-      rb = old;
-    } else {
-      const int32_t old = atomicCAS(&parent[ra], ra, rb);
-      if (old == ra) break;
-      ra = old;
-    }
-  }
-}
-
 // For each non-degenerate edge (a,b) of face f: every face g > f among a's incident faces that also has a corner at b
 // shares the edge {a,b} with f (any two distinct corners of a triangle are joined by one of its edges).
 __global__ void __launch_bounds__(CL_THREADS) clean_union_kernel(const int32_t* __restrict__ faces, int64_t nf,

@@ -339,6 +339,32 @@ class Engine:
             check(self.lib.disn_mc_fetch(self._h, verts.ctypes.data_as(C.c_void_p), faces.ctypes.data_as(C.c_void_p)))
         return (verts, faces, labels) if want_labels else (verts, faces)
 
+    def mesh_sdf(self, res: int, bbox=None, expand_rate: float = 1.2, sigma: float = 0.0, verts=None, faces=None,
+                 device_ptr: int | None = None):
+        """Signed distance field of the resident mesh (preprocessing/create_point_sdf_grid.py:200-210,
+        computeDistanceField -s): (res+1)^3 grid over bbox (None = cube around the mesh AABB scaled by expand_rate),
+        sign by exterior flood fill with wall threshold sigma (the reference's -g).  verts/faces, if given, are loaded
+        first.  -> (grid [R,R,R] float32 (z,y,x), or None when written to device_ptr, bbox as a list of 6 floats)."""
+        if verts is not None or faces is not None:
+            self.load_mesh(verts, faces)
+        R = res + 1
+        bb = None if bbox is None else (C.c_double * 6)(*[float(v) for v in bbox])
+        used = (C.c_double * 6)()
+        if device_ptr is None:
+            ok = res >= 1 and R ** 3 < 2 ** 31       # otherwise the library reports the bad resolution
+            out = np.empty((R, R, R) if ok else (1,), np.float32)
+            ptr, flags = out.ctypes.data_as(C.c_void_p), 0
+        else:
+            out, ptr, flags = None, C.c_void_p(device_ptr), DISN_DEVICE_PTR
+        check(self.lib.disn_mesh_sdf(self._h, res, bb, float(expand_rate), float(sigma), ptr, used, flags))
+        return out, list(used)
+
+    def mesh_sdf_phase_ms(self):
+        """Milliseconds of the last mesh_sdf's phases: BVH build, distance, edge rasterisation, flood fill and sign."""
+        ms = (C.c_float * 4)()
+        check(self.lib.disn_mesh_sdf_phase_ms(self._h, ms))
+        return dict(zip(("build", "distance", "rasterise", "flood"), list(ms)))
+
     def eval_grid_resident(self, sdf_params, trans_mat, sdf_res: int) -> int:
         """Whole [B,R,R,R] grid evaluated into the context's HBM buffer; returns its device address."""
         sp = np.ascontiguousarray(sdf_params, dtype=np.float64).reshape(-1, 6)

@@ -22,6 +22,8 @@
  *                                       (test/create_sdf.py:319-323)
  *   disn_mesh_load / disn_mesh_clean <-> clean_single_mesh (postprocessing/clean_smallparts.py:38-54):
  *                                       pymesh.separate_mesh, keep rule, pymesh.merge_meshes
+ *   disn_mesh_sdf                   <-> os.system("computeDistanceField <obj> res res res -s -e <e> -o X.dist -m 1 [-g s]")
+ *                                       (preprocessing/create_point_sdf_grid.py:200-210)
  *
  * Conventions: every function returns 0 on success, non-zero on failure with a thread-local message
  * in disn_last_error(); the caller owns all buffers; all tensors are float32, row-major, NHWC / [B,N,C]
@@ -147,6 +149,20 @@ int disn_fetch(disn_ctx* ctx, const void* dev, void* host, int64_t bytes);
 int disn_mesh_load(disn_ctx* ctx, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces);
 int disn_mesh_clean(disn_ctx* ctx, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
                     int64_t* n_kept, int64_t* n_verts, int64_t* n_faces);
+
+/* Signed distance field of the resident mesh (disn_mesh_load / disn_mc_run / disn_mesh_clean), the reference's
+ * computeDistanceField -s (preprocessing/create_point_sdf_grid.py:200-210): R = res+1 points per axis over bbox
+ * (NULL = cube around the mesh AABB scaled by expand_rate; the box used is written to bbox_out[6] if non-NULL),
+ * sign by exterior flood fill with wall threshold sigma.  out: host float[R,R,R] (z,y,x), or a device pointer
+ * with DISN_DEVICE_PTR (e.g. straight into disn_mc_run).  Grid points are disn_eval_grid's (float64 linspace cast to
+ * float32); distances are exact point-triangle distances in float64 rounded once to float32; a point is exterior when
+ * it is farther than sigma from the mesh and connected to the box boundary through grid edges that cross no face
+ * (DESIGN.md 4.7).  The call synchronises with the context's stream.
+ * disn_mesh_sdf_phase_ms: milliseconds of the last call's four phases (BVH build, distance, edge rasterisation, flood
+ * fill and sign) into ms[4]. */
+int disn_mesh_sdf(disn_ctx* ctx, int32_t res, const double* bbox, double expand_rate, double sigma, float* out,
+                  double* bbox_out, uint32_t flags);
+int disn_mesh_sdf_phase_ms(disn_ctx* ctx, float* ms);
 
 /* Estimated-camera path (reference: demo/demo.py:195-258 cam_evl, cam_est/model_cam.py:47-109, models/posenet.py:91-124):
  * imgs host [B,H,W,3] -> VGG-16 embedding (the context's `vgg_16/...` weights = the camera checkpoint's) -> three FC
