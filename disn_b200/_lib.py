@@ -62,6 +62,13 @@ EXPORTS = {
     "disn_mesh_sdf": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_double, C.c_double, C.c_void_p,
                                 C.POINTER(C.c_double), C.c_uint32]),
     "disn_mesh_sdf_phase_ms": (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
+    "disn_mesh_part_areas": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int32)]),
+    "disn_mesh_normalize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                      C.c_void_p, C.POINTER(C.c_double), C.c_void_p]),
+    "disn_field": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),
+    "disn_sdf_band_count": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_uint32, C.c_void_p]),
+    "disn_sdf_band_gather": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "disn_sdf_strided": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_uint32, C.c_void_p]),
     "disn_fetch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]),
     "disn_shared_alloc": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_void_p), C.c_char_p]),
     "disn_shared_open": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

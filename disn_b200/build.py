@@ -10,12 +10,14 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdisn_b200.so")
 TEST_LIB = os.path.join(HERE, "libdisn_b200_test.so")
 SOURCES = ["api.cu", "encoder.cu", "point_fp32.cu", "point_tc.cu", "mc.cu", "chamfer.cu", "conv_tc.cu", "cam.cu", "iou.cu",
-           "decoder.cu", "emd.cu", "mesh_clean.cu", "mesh_sdf.cu"]
+           "decoder.cu", "emd.cu", "mesh_clean.cu", "mesh_sdf.cu", "mesh_normalize.cu", "sdf_sample.cu"]
 # diagnostics: selftests / probes, plus encoder.cu rebuilt with its debug GEMM harness -> libdisn_b200_test.so
 DIAG_SOURCES = ["tc_selftest.cu", "tc_probe.cu"]
 # voxel classification (iou.cu), the small-part keep rule (mesh_clean.cu) and the distances and edge crossings of the
-# signed distance field (mesh_sdf.cu) must match the float64 oracle operation for operation
-EXTRA_FLAGS = {"iou.cu": ["--fmad=false"], "mesh_clean.cu": ["--fmad=false"], "mesh_sdf.cu": ["--fmad=false"]}
+# signed distance field (mesh_sdf.cu) and the face areas, surface samples and normalised vertices (mesh_normalize.cu) must
+# match the float64 oracle operation for operation
+EXTRA_FLAGS = {"iou.cu": ["--fmad=false"], "mesh_clean.cu": ["--fmad=false"], "mesh_sdf.cu": ["--fmad=false"],
+               "mesh_normalize.cu": ["--fmad=false"]}
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC,-ffp-contract=off", "--expt-relaxed-constexpr", "-shared"]

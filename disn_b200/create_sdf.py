@@ -228,6 +228,34 @@ def read_obj(path):
             np.array(faces, np.int64).astype(np.int32).reshape(-1, 3))
 
 
+def read_obj_parts(path):
+    """read_obj plus the parts trimesh.load_mesh(process=False) splits an OBJ into (restated, unpinned: one part per
+    `usemtl` material name, in order of first appearance; faces before the first `usemtl`, or every face of a file
+    without one, form their own part) -> (verts [V,3] float32, faces [F,3] int32 0-based, part_ids [F] int32,
+    names: one material name, or None, per part).  The vertex array is shared by all parts."""
+    verts, faces, pids, names, index = [], [], [], [], {}
+    cur = None
+    with open(path) as fh:
+        for n, line in enumerate(fh, 1):
+            tok = line.split()
+            if not tok:
+                continue
+            if tok[0] == "v":
+                verts.append([float(x) for x in tok[1:4]])
+            elif tok[0] == "usemtl":
+                cur = tok[1] if len(tok) > 1 else ""
+            elif tok[0] == "f":
+                if len(tok) != 4:
+                    raise ValueError("%s:%d: only triangle faces are supported, found %d corners" % (path, n, len(tok) - 1))
+                if cur not in index:
+                    index[cur] = len(names)
+                    names.append(cur)
+                faces.append([int(t.split("/")[0]) - 1 for t in tok[1:]])
+                pids.append(index[cur])
+    return (np.array(verts, np.float64).astype(np.float32).reshape(-1, 3),
+            np.array(faces, np.int64).astype(np.int32).reshape(-1, 3), np.array(pids, np.int32), names)
+
+
 def create_one_cube_obj(marching_cube_command, i, sdf_file, cube_obj_file):
     """test/create_sdf.py:319-323.  The reference runs `<marching_cube_command> <dist> <obj> -i <iso>` (a
     closed-source CPU binary); here the .dist is meshed by the CUDA marching-cubes post-pass.

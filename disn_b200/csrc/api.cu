@@ -536,6 +536,61 @@ int disn_mesh_sdf_phase_ms(disn_ctx* c, float* ms) {
   return 0;
 }
 
+int disn_mesh_part_areas(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, int64_t* part_q, int32_t* shift) {
+  DISN_REQUIRE(c, "null ctx");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  return mesh_part_areas(c, part_ids, n_parts, part_q, shift);
+}
+
+int disn_mesh_normalize(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, const int64_t* amounts,
+                        const double* draws, int64_t n_draws, const double* given, double* centroid, double* m,
+                        double* samples) {
+  DISN_REQUIRE(c, "null ctx");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  return mesh_normalize(c, part_ids, n_parts, amounts, draws, n_draws, given, centroid, m, samples);
+}
+
+int disn_field(disn_ctx* c, int32_t R, float** out_dev) {
+  DISN_REQUIRE(c && out_dev, "null argument");
+  DISN_REQUIRE(R >= 2 && (int64_t)R * R * R <= INT32_MAX, "field: 2 <= R and R^3 < 2^31");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  if (c->d_field.ensure((size_t)R * R * R * sizeof(float))) return -1;
+  *out_dev = c->d_field.as<float>();
+  return 0;
+}
+
+int disn_sdf_band_count(disn_ctx* c, const float* sdf, int32_t R, float iso, const float* edges, uint32_t flags,
+                        int64_t* counts) {
+  DISN_REQUIRE(c && sdf && edges && counts, "null argument");
+  DISN_REQUIRE(R >= 2 && (int64_t)R * R * R < INT32_MAX, "sdf_band_count: 2 <= R and R^3 < 2^31 - 1");
+  // the four index lists share one buffer of R^3 entries: it holds them all only when no point lies in two bands
+  for (int a = 0; a < 4; ++a) {
+    const float la = edges[2 * a], ha = edges[2 * a + 1];
+    DISN_REQUIRE(!std::isnan(la) && !std::isnan(ha), "sdf_band_count: band edges must not be NaN");
+    for (int b = a + 1; b < 4; ++b) {
+      const float lb = edges[2 * b], hb = edges[2 * b + 1];
+      const bool empty = !(la < ha) || !(lb < hb);
+      DISN_REQUIRE(empty || ha <= lb || hb <= la,
+                   "sdf_band_count: bands " + std::to_string(a) + " and " + std::to_string(b) + " overlap");
+    }
+  }
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  return band_count(c, sdf, R, iso, edges, (flags & DISN_DEVICE_PTR) != 0, counts);
+}
+
+int disn_sdf_band_gather(disn_ctx* c, const float* axes, const int64_t* choices, const int64_t* k, float* out) {
+  DISN_REQUIRE(c && axes && k && ((choices && out) || k[0] + k[1] + k[2] + k[3] == 0), "null argument");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  return band_gather(c, axes, choices, k, out);
+}
+
+int disn_sdf_strided(disn_ctx* c, const float* sdf, int32_t R, int32_t reduce, uint32_t flags, float* out) {
+  DISN_REQUIRE(c && sdf && out, "null argument");
+  DISN_REQUIRE(R >= 2 && (int64_t)R * R * R <= INT32_MAX && reduce >= 1, "sdf_strided: 2 <= R, R^3 < 2^31, reduce >= 1");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  return sdf_strided(c, sdf, R, reduce, (flags & DISN_DEVICE_PTR) != 0, out);
+}
+
 int disn_eval_grid_resident(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t B, int32_t sdf_res,
                             float** out_dev) {
   DISN_REQUIRE(c && sdf_params && trans_mat && out_dev, "null argument");

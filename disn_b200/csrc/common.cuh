@@ -242,6 +242,18 @@ struct disn_ctx {
   disn::PinnedBuffer sdf_host;
   cudaEvent_t sdf_ev[5] = {};
   float sdf_phase_ms[4] = {};
+  // resident field of the preprocessing chain (disn_field): mesh_sdf writes it, marching cubes and the samplers read it
+  disn::DevBuffer d_field;
+  // surface-sample normalisation (mesh_normalize.cu): scratch arena and pinned statistics words
+  disn::DevBuffer nm_arena;
+  disn::PinnedBuffer nm_host;
+  // band / strided sampling of a field (sdf_sample.cu): host-field staging, flags and scan scratch, the four compacted
+  // index lists, their counts, and the gather staging; smp_src / smp_R / smp_n describe the lists of the last band count
+  disn::DevBuffer smp_in, smp_flag, smp_scan, smp_list, smp_counts, smp_gather;
+  disn::PinnedBuffer smp_host;
+  const float* smp_src = nullptr;
+  int32_t smp_R = 0;
+  int64_t smp_n[4] = {};
   // device-resident SDF grid of disn_eval_grid_resident and host staging for the marching-cubes input
   disn::DevBuffer d_grid;
   disn::DevBuffer d_mc_in;
@@ -292,6 +304,14 @@ int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face
 // mesh_sdf.cu
 int mesh_sdf(disn_ctx* c, int32_t res, const double* bbox, double expand_rate, double sigma, float* out,
              double* bbox_out, bool device_out);
+// mesh_normalize.cu
+int mesh_part_areas(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, int64_t* part_q, int32_t* shift);
+int mesh_normalize(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, const int64_t* amounts, const double* draws,
+                   int64_t n_draws, const double* given, double* centroid_out, double* m_out, double* samples_out);
+// sdf_sample.cu
+int band_count(disn_ctx* c, const float* sdf, int32_t R, float iso, const float* edges, bool device_ptr, int64_t* counts);
+int band_gather(disn_ctx* c, const float* axes, const int64_t* choices, const int64_t* k, float* out);
+int sdf_strided(disn_ctx* c, const float* sdf, int32_t R, int32_t reduce, bool device_ptr, float* out);
 // api.cu: numpy.linspace(start, stop, num) in float64 cast to float32 (the grid coordinates of eval_grid and mesh_sdf)
 void axis_table(double start, double stop, int num, float* out);
 }  // namespace disn

@@ -44,6 +44,7 @@ class Engine:
         check(self.lib.disn_create(C.byref(cfg), C.byref(self._h)))
         self.batch = 0
         self._mesh_faces = 0        # face count of the resident mesh (sizes clean_mesh's labels)
+        self._mesh_verts = 0        # vertex count of the resident mesh (sizes fetch_mesh)
         self.last_clean = None
 
     # -- lifetime -----------------------------------------------------------------------------
@@ -299,6 +300,7 @@ class Engine:
         nv, nf = C.c_int64(0), C.c_int64(0)
         check(self.lib.disn_mc_run(self._h, ptr, R, bb, float(iso), flags, C.byref(nv), C.byref(nf)))
         self._mesh_faces = nf.value
+        self._mesh_verts = nv.value
         if not fetch:
             return nv.value, nf.value
         verts = np.empty((nv.value, 3), dtype=np.float32)
@@ -318,6 +320,15 @@ class Engine:
         f = np.ascontiguousarray(faces, np.int32).reshape(-1, 3)
         check(self.lib.disn_mesh_load(self._h, v.ctypes.data_as(C.c_void_p), len(v), f.ctypes.data_as(C.c_void_p), len(f)))
         self._mesh_faces = len(f)
+        self._mesh_verts = len(v)
+
+    def fetch_mesh(self):
+        """The resident mesh (last marching_cubes / load_mesh / clean_mesh / normalize_mesh) -> (verts, faces)."""
+        verts = np.empty((self._mesh_verts, 3), dtype=np.float32)
+        faces = np.empty((self._mesh_faces, 3), dtype=np.int32)
+        if len(verts) or len(faces):        # the library copies each array only when the resident mesh has entries
+            check(self.lib.disn_mc_fetch(self._h, verts.ctypes.data_as(C.c_void_p), faces.ctypes.data_as(C.c_void_p)))
+        return verts, faces
 
     def clean_mesh(self, dist_thresh: float = 0.5, num_thresh: float = 0.3, fetch: bool = True, want_labels: bool = False):
         """postprocessing/clean_smallparts.py:38-54 on the resident mesh, in place: drop every edge-connected component
@@ -330,6 +341,7 @@ class Engine:
                                        None if labels is None else labels.ctypes.data_as(C.c_void_p),
                                        C.byref(nc), C.byref(nk), C.byref(nv), C.byref(nf)))
         self._mesh_faces = nf.value
+        self._mesh_verts = nv.value
         self.last_clean = MeshCleanCounts(nv.value, nf.value, nc.value, nk.value)
         if not fetch:
             return (self.last_clean, labels) if want_labels else self.last_clean
@@ -364,6 +376,105 @@ class Engine:
         ms = (C.c_float * 4)()
         check(self.lib.disn_mesh_sdf_phase_ms(self._h, ms))
         return dict(zip(("build", "distance", "rasterise", "flood"), list(ms)))
+
+    # -- per-object preprocessing: normalisation and field samples ------------------------------------------------
+    def part_areas(self, part_ids=None, n_parts: int = 1):
+        """Quantised part areas of the resident mesh (DESIGN.md §4.8): part_ids [n_faces] in [0, n_parts) or None (one
+        part) -> (Q_p int64 [n_parts], shift s); Q_p is the exact sum of rint(area_f * 2^s) over the part's faces."""
+        pid = None if part_ids is None else np.ascontiguousarray(part_ids, np.int32)
+        q = np.empty(n_parts, np.int64)
+        s = C.c_int32(0)
+        check(self.lib.disn_mesh_part_areas(self._h, None if pid is None else pid.ctypes.data_as(C.c_void_p), n_parts,
+                                            q.ctypes.data_as(C.c_void_p), C.byref(s)))
+        return q, s.value
+
+    def normalize_mesh(self, part_ids=None, n_parts: int = 1, amounts=None, draws=None, given=None,
+                       want_samples: bool = False):
+        """preprocessing/create_point_sdf_grid.py:169-198 get_normalize_mesh on the resident mesh: amounts [n_parts] and
+        draws [N,3] = (face pick, r1, r2) in sample_surface's np.random order -> (centroid float64 [3], m) and, with
+        want_samples, the surface samples [N,3] float64.  The resident vertices become float32((v - c) / m).
+        given = (cx, cy, cz, m) skips the sampling and only transforms the vertices."""
+        c, m = np.empty(3, np.float64), C.c_double(0.0)
+        ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+        if given is not None:
+            g = np.ascontiguousarray(np.asarray(given, np.float64).reshape(4))
+            check(self.lib.disn_mesh_normalize(self._h, None, 1, None, None, 0, ptr(g), ptr(c), C.byref(m), None))
+            return c, m.value
+        pid = None if part_ids is None else np.ascontiguousarray(part_ids, np.int32)
+        amt = np.ascontiguousarray(amounts, np.int64).reshape(-1)
+        dr = np.ascontiguousarray(draws, np.float64).reshape(-1, 3)
+        smp = np.empty((len(dr), 3), np.float64) if want_samples else None
+        check(self.lib.disn_mesh_normalize(self._h, ptr(pid), n_parts, ptr(amt), ptr(dr), len(dr), None, ptr(c),
+                                           C.byref(m), ptr(smp)))
+        return (c, m.value, smp) if want_samples else (c, m.value)
+
+    def field_buffer(self, R: int) -> int:
+        """Device address of the context's resident [R,R,R] field (grows only; valid until a larger request)."""
+        out = C.c_void_p()
+        check(self.lib.disn_field(self._h, R, C.byref(out)))
+        return int(out.value)
+
+    def band_samples(self, num_sample: int, bandwidth: float, iso_val: float, params, sdf_res: int, sdf=None,
+                     device_ptr: int | None = None):
+        """preprocessing/create_point_sdf_grid.py:74-113 sample_sdf on the device, bit for bit the host function for the
+        same np.random state: the four bands of float32(sdf - iso) are compacted in HBM, the host applies the carry-over
+        rule and draws np.random.randint exactly as the host function does, the device gathers the [n,4] rows.
+        params: the float32 box of get_sdf; sdf: host [R,R,R] float32, or device_ptr (e.g. field_buffer).
+        iso_val and bandwidth are taken as Python floats, as the reference passes them: numpy 2 then subtracts and
+        compares in float32 (NEP 50), which is what the device does.  A float64 numpy scalar would make the host
+        function compute in float64 instead, so both are converted with float() here and in the package's callers."""
+        R = sdf_res + 1
+        bw = float(bandwidth)
+        iso_val = float(iso_val)
+        percentages = [[-1. * bw, -1. * bw * 0.30, int(num_sample * 0.25)],
+                       [-1. * bw * 0.30, 0, int(num_sample * 0.25)],
+                       [0, bw * 0.30, int(num_sample * 0.25)],
+                       [bw * 0.30, bw, int(num_sample * 0.25)]]
+        edges = np.array([[p[0], p[1]] for p in percentages], np.float64).astype(np.float32)
+        if device_ptr is None:
+            a = _f32(sdf)
+            assert a.size == R ** 3
+            src, flags = a.ctypes.data_as(C.c_void_p), 0
+        else:
+            src, flags = C.c_void_p(device_ptr), DISN_DEVICE_PTR
+        counts = np.zeros(4, np.int64)
+        check(self.lib.disn_sdf_band_count(self._h, src, R, float(np.float32(iso_val)), edges.ctypes.data_as(C.c_void_p),
+                                           flags, counts.ctypes.data_as(C.c_void_p)))
+        k = np.zeros(4, np.int64)
+        choices = []
+        for i in range(4):
+            n = int(counts[i])
+            if n < percentages[i][2]:
+                if i < 3:
+                    percentages[i + 1][2] += percentages[i][2] - n
+                percentages[i][2] = n
+            if n == 0:
+                continue
+            choices.append(np.random.randint(n, size=percentages[i][2]).astype(np.int64))
+            k[i] = percentages[i][2]
+        ch = np.ascontiguousarray(np.concatenate(choices) if choices else np.zeros(0, np.int64))
+        p = np.asarray(params, np.float32)
+        axes = np.ascontiguousarray(np.concatenate(
+            [np.linspace(p[a], p[3 + a], num=R).astype(np.float32) for a in range(3)]))
+        out = np.empty((len(ch), 4), np.float32)
+        check(self.lib.disn_sdf_band_gather(self._h, axes.ctypes.data_as(C.c_void_p), ch.ctypes.data_as(C.c_void_p),
+                                            k.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))
+        self.last_band_counts = counts
+        return out
+
+    def sdf_strided(self, R: int, reduce: int, sdf=None, device_ptr: int | None = None):
+        """create_point_sdf_fullgrid.py:70-96: every reduce-th value of the [R,R,R] field on each axis -> [M,M,M],
+        M = (R-1)//reduce + 1."""
+        M = (R - 1) // reduce + 1 if reduce >= 1 else 1
+        out = np.empty((M, M, M), np.float32)
+        if device_ptr is None:
+            a = _f32(sdf)
+            assert a.size == R ** 3
+            src, flags = a.ctypes.data_as(C.c_void_p), 0
+        else:
+            src, flags = C.c_void_p(device_ptr), DISN_DEVICE_PTR
+        check(self.lib.disn_sdf_strided(self._h, src, R, reduce, flags, out.ctypes.data_as(C.c_void_p)))
+        return out
 
     def eval_grid_resident(self, sdf_params, trans_mat, sdf_res: int) -> int:
         """Whole [B,R,R,R] grid evaluated into the context's HBM buffer; returns its device address."""

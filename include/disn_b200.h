@@ -24,6 +24,10 @@
  *                                       pymesh.separate_mesh, keep rule, pymesh.merge_meshes
  *   disn_mesh_sdf                   <-> os.system("computeDistanceField <obj> res res res -s -e <e> -o X.dist -m 1 [-g s]")
  *                                       (preprocessing/create_point_sdf_grid.py:200-210)
+ *   disn_mesh_part_areas / disn_mesh_normalize <-> get_normalize_mesh (preprocessing/create_point_sdf_grid.py:169-198)
+ *   disn_field / disn_sdf_band_count / disn_sdf_band_gather <-> the field between create_one_sdf, create_one_cube_obj
+ *                                       and sample_sdf (:74-113, :200-252); disn_sdf_strided <-> the strided sample_sdf
+ *                                       of create_point_sdf_fullgrid.py:70-96
  *
  * Conventions: every function returns 0 on success, non-zero on failure with a thread-local message
  * in disn_last_error(); the caller owns all buffers; all tensors are float32, row-major, NHWC / [B,N,C]
@@ -163,6 +167,47 @@ int disn_mesh_clean(disn_ctx* ctx, double dist_thresh, double num_thresh, int32_
 int disn_mesh_sdf(disn_ctx* ctx, int32_t res, const double* bbox, double expand_rate, double sigma, float* out,
                   double* bbox_out, uint32_t flags);
 int disn_mesh_sdf_phase_ms(disn_ctx* ctx, float* ms);
+
+/* Surface-sample normalisation of the resident mesh, the reference's get_normalize_mesh
+ * (preprocessing/create_point_sdf_grid.py:169-198: per-part sample counts int32(area_i * 16384 / area_sum) at :172-189,
+ * trimesh.sample.sample_surface, centroid and max norm of the samples, (v - c) / m).  Definitions (DESIGN.md 4.8): face
+ * areas in float64, quantised to int64 Q_f = rint(a_f * 2^shift) and scanned exactly per part.
+ *   disn_mesh_part_areas: part_ids host int32 [n_faces] in [0, n_parts) (NULL: one part) -> part_q [n_parts] (the part
+ *     totals of Q_f) and the shift.  The caller derives the amounts n_p = floor(Q_p * 16384 / sum Q) and draws the
+ *     random numbers in sample_surface's order.
+ *   disn_mesh_normalize: amounts [n_parts], draws host double [n_draws][3] = (face pick, r1, r2) per sample, parts in
+ *     order, n_draws = sum of the amounts; writes centroid [3] and m (float64, the reference's norm_params) and the
+ *     samples [n_draws][3] float64 if non-NULL, and replaces the resident vertices by float32((v - c) / m).  given:
+ *     NULL, or double[4] = (c, m) to skip the sampling and only transform the vertices
+ *     (create_point_sdf_fullgrid.py:163-183, where part_ids / amounts / draws are ignored).
+ * Errors leave the resident mesh unchanged: no faces, n_parts outside [1, n_faces], non-finite vertices, a part id out of
+ * range, an amount outside [0, 2^31), an amount on a zero-area part, a draw count that differs from the amounts' sum, no samples, draws outside [0, 1),
+ * max |sample| * n_draws >= 2^30 (int64 range of the centroid sums) or m = 0. */
+int disn_mesh_part_areas(disn_ctx* ctx, const int32_t* part_ids, int32_t n_parts, int64_t* part_q, int32_t* shift);
+int disn_mesh_normalize(disn_ctx* ctx, const int32_t* part_ids, int32_t n_parts, const int64_t* amounts,
+                        const double* draws, int64_t n_draws, const double* given, double* centroid, double* m,
+                        double* samples);
+
+/* Resident field of the per-object preprocessing chain (preprocessing/create_point_sdf_grid.py:213-246): a context-owned
+ * device buffer of R^3 floats (valid until the next disn_field call with a larger R), passed with DISN_DEVICE_PTR to
+ * disn_mesh_sdf (write), disn_mc_run (create_one_cube_obj, :248-252) and the samplers below, so the field never leaves
+ * HBM except as samples. */
+int disn_field(disn_ctx* ctx, int32_t R, float** out_dev);
+
+/* Band sampling, the reference's sample_sdf (preprocessing/create_point_sdf_grid.py:74-113), in two calls around the
+ * host's np.random.randint draws:
+ *   disn_sdf_band_count: sdf [R,R,R] (host, or device with DISN_DEVICE_PTR; a device field must stay valid until the
+ *     gather), iso and edges [4][2] = (lo, hi) as float32 -> counts [4] of the points with lo <= float32(sdf - iso) < hi;
+ *     each band's flat indices are kept on the device in ascending order.  The bands must be disjoint (the four lists
+ *     share one buffer of R^3 entries): NaN edges or two non-empty intervals that overlap are an error;
+ *   disn_sdf_band_gather: axes host float [3][R] (the x, y, z tables of the host function), choices host int64 (k[0]
+ *     indices into band 0, then band 1, ...) -> out [sum k][4] float32 rows (x, y, z, sdf).
+ * Strided sampling, create_point_sdf_fullgrid.py:70-96: out [M,M,M] with M = (R-1)/reduce + 1 holds every reduce-th
+ * value on each axis. */
+int disn_sdf_band_count(disn_ctx* ctx, const float* sdf, int32_t R, float iso, const float* edges, uint32_t flags,
+                        int64_t* counts);
+int disn_sdf_band_gather(disn_ctx* ctx, const float* axes, const int64_t* choices, const int64_t* k, float* out);
+int disn_sdf_strided(disn_ctx* ctx, const float* sdf, int32_t R, int32_t reduce, uint32_t flags, float* out);
 
 /* Estimated-camera path (reference: demo/demo.py:195-258 cam_evl, cam_est/model_cam.py:47-109, models/posenet.py:91-124):
  * imgs host [B,H,W,3] -> VGG-16 embedding (the context's `vgg_16/...` weights = the camera checkpoint's) -> three FC
