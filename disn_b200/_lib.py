@@ -52,6 +52,10 @@ EXPORTS = {
     "disn_launch_count": (C.c_int64, [C.c_void_p]),
     "disn_eval_grid_resident": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_int32, C.c_int32,
                                           C.POINTER(C.c_void_p)]),
+    "disn_eval_grid_indexed": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                         C.c_int64, C.c_void_p, C.c_uint32]),
+    "disn_eval_grid_adaptive": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_int32, C.c_int32, C.c_float,
+                                          C.c_double, C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_int32)]),
     "disn_mc_run": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_float, C.c_uint32,
                               C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "disn_mc_fetch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -93,6 +97,10 @@ TEST_EXPORTS = {
     "disn_tc_selftest": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "disn_tc_selftest_mixed": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                          C.c_void_p, C.c_void_p]),
+    "disn_adaptive_mask": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    "disn_adaptive_from_field": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_float, C.c_double,
+                                           C.c_uint32, C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_int32)]),
+    "disn_adaptive_phase_ms": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]),
 }
 
 _lib = None

@@ -129,6 +129,9 @@ def test_one_epoch(sess, ops, batches):
     No .dist round trip through the file system; FLAGS.keep_dist=True also writes the reference's .dist artefact.
     FLAGS.clean_smallparts=True runs the reference's postprocessing/clean_smallparts.py step on each mesh while it is
     still in HBM (thresholds FLAGS.clean_dist_thresh / clean_num_thresh, default 0.5 / 0.3).
+    FLAGS.adaptive=True (default False) replaces the batch's dense grid with one coarse-to-fine grid per image
+    (Engine.eval_grid_adaptive, band FLAGS.adaptive_band, default 1.0): the network runs only near the surface; output
+    names, cleaning, keep_dist and the OBJ writer are unchanged.
     The reference's literal loop (host grid, SPLIT_SIZE chunks through sess.run, reassembly, /SDF_WEIGHT) is kept as a
     verification aid in tests/reference_loop.py."""
     log_string(str(datetime.now()))
@@ -140,12 +143,19 @@ def test_one_epoch(sess, ops, batches):
             with _ENGINE_LOCK:
                 sess.engine.encode(batch_data["img"])
                 sess._img_key = None
-                grid_ptr = sess.engine.eval_grid_resident(batch_data["sdf_params"], batch_data["trans_mat"], FLAGS.sdf_res)
+                adaptive = getattr(FLAGS, "adaptive", False)
+                if not adaptive:
+                    grid_ptr = sess.engine.eval_grid_resident(batch_data["sdf_params"], batch_data["trans_mat"], FLAGS.sdf_res)
                 for b in range(BATCH_SIZE):
                     print("{}/{}, submit create_obj {}, {}, {}".format(batch_idx, "?", batch_data["cat_id"][b],
                                                                        batch_data["obj_nm"][b], batch_data["view_id"][b]))
                     path = obj_path(RESULT_OBJ_PATH, batch_data["cat_id"][b], batch_data["obj_nm"][b], batch_data["view_id"][b])
-                    dev = grid_ptr + b * R * R * R * 4
+                    if adaptive:        # coarse-to-fine grid of this image (DESIGN.md §4.9), meshed before the next one
+                        dev, _ = sess.engine.eval_grid_adaptive(
+                            np.asarray(batch_data["sdf_params"], np.float64)[b], np.asarray(batch_data["trans_mat"])[b],
+                            FLAGS.sdf_res, iso=float(FLAGS.iso), band=float(getattr(FLAGS, "adaptive_band", 1.0)), image=b)
+                    else:
+                        dev = grid_ptr + b * R * R * R * 4
                     if getattr(FLAGS, "clean_smallparts", False):
                         # postprocessing/clean_smallparts.py on the resident mesh before it leaves HBM
                         sess.engine.marching_cubes(None, batch_data["sdf_params"][b], float(FLAGS.iso), device_ptr=dev,

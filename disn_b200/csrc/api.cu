@@ -18,6 +18,8 @@ disn_ctx::~disn_ctx() {
   encoder_graph_reset(this);
   for (cudaEvent_t e : sdf_ev)
     if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : ad_ev)
+    if (e) cudaEventDestroy(e);
   if (own_stream && stream) cudaStreamDestroy(stream);
 }
 
@@ -89,6 +91,10 @@ static int check_status(disn_ctx* c) {
   if (st & DISN_STATUS_FP16_OVERFLOW) {
     set_error("DISN_PREC_F16F8: an MLP activation exceeded the fp16 range (65504); the result is invalid -- "
               "use DISN_PREC_BF16X3 (fp32 range) for these weights");
+    return -4;
+  }
+  if (st & DISN_STATUS_BAD_INDEX) {
+    set_error("eval_grid_indexed: a grid index lies outside [0, (sdf_res+1)^3); the result is invalid");
     return -4;
   }
   set_error("kernel reported status " + std::to_string(st));
@@ -249,7 +255,12 @@ int disn::run_point_job(disn_ctx* c, PointJob& job) {
   fill_stream(c, "sdfprediction", job.g);
   fill_stream(c, "sdfprediction_imgfeat", job.l);
   job.status = c->d_status.as<int>();
-  if (c->cfg.precision == DISN_PREC_FP32) return launch_point_fp32(c, job);
+  if (c->cfg.precision == DISN_PREC_FP32) {
+    if (launch_point_fp32(c, job)) return -1;
+    if (job.idx)      // only an indexed job can raise a status on the fp32 path
+      DISN_CUDA_OK(cudaMemcpyAsync(c->h_status.as<int>(), job.status, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    return 0;
+  }
   if (launch_point_tc(c, job)) return -1;
   // the status word travels to the pinned mirror behind the kernel; whoever synchronises next checks it
   DISN_CUDA_OK(cudaMemcpyAsync(c->h_status.as<int>(), job.status, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -324,23 +335,7 @@ int disn_eval_grid(disn_ctx* c, const double* sdf_params, const float* trans_mat
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
   const int64_t N = (int64_t)(z1 - z0) * R * R;
   if (N == 0) return 0;
-  // axis tables (host float64 linspace -> float32), uploaded per call: B*3*R floats
-  const size_t axes_bytes = (size_t)8 * 3 * R * sizeof(float);
-  if (axes_bytes > c->d_axes.bytes()) c->axes_key.clear();   // a new allocation holds no tables yet
-  if (c->d_axes.ensure(axes_bytes)) return -1;
-  // re-upload only when the boxes / resolution change (keeps repeated calls free of host syncs)
-  std::vector<double> key(sdf_params, sdf_params + (size_t)B * 6);
-  key.push_back((double)R);
-  if (key != c->axes_key) {
-    std::vector<float> axes((size_t)B * 3 * R);
-    for (int b = 0; b < B; ++b)
-      for (int a = 0; a < 3; ++a)
-        linspace_f32(sdf_params[b * 6 + a], sdf_params[b * 6 + 3 + a], R, &axes[((size_t)b * 3 + a) * R]);
-    DISN_CUDA_OK(cudaMemcpyAsync(c->d_axes.as<float>(), axes.data(), axes.size() * sizeof(float), cudaMemcpyHostToDevice,
-                                 c->stream));
-    DISN_CUDA_OK(cudaStreamSynchronize(c->stream));   // `axes` is a stack-owned staging buffer
-    c->axes_key = key;
-  }
+  if (grid_axes(c, sdf_params, B, R)) return -1;
 
   PointJob job{};
   job.B = B; job.N = N; job.R = R; job.z0 = z0; job.axes = c->d_axes.as<float>();
@@ -606,6 +601,52 @@ int disn_eval_grid_resident(disn_ctx* c, const double* sdf_params, const float* 
   return 0;
 }
 
+int disn_eval_grid_indexed(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t image, int32_t sdf_res,
+                           const int32_t* idx, int64_t n, float* out, uint32_t flags) {
+  DISN_REQUIRE(c && sdf_params && trans_mat && ((idx && out) || n == 0), "null argument");
+  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(image >= 0 && image < c->enc_B, "image outside the encoded batch");
+  DISN_REQUIRE(sdf_res >= 1 && (int64_t)(sdf_res + 1) * (sdf_res + 1) * (sdf_res + 1) <= INT32_MAX,
+               "eval_grid_indexed: 1 <= sdf_res and (sdf_res+1)^3 < 2^31");
+  DISN_REQUIRE(n >= 0, "negative n");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  if (n == 0) return 0;
+  const int R = sdf_res + 1;
+  if (grid_axes(c, sdf_params, 1, R)) return -1;
+  if (flags & DISN_DEVICE_PTR) return eval_indexed(c, image, R, trans_mat, idx, n, out);
+  const int64_t R3 = (int64_t)R * R * R;
+  for (int64_t i = 0; i < n; ++i)
+    DISN_REQUIRE(idx[i] >= 0 && idx[i] < R3, "eval_grid_indexed: index " + std::to_string(idx[i]) + " at position " +
+                                                 std::to_string(i) + " lies outside [0, (sdf_res+1)^3)");
+  if (c->d_idx.ensure((size_t)n * sizeof(int32_t)) || ensure_point_scratch(c, n)) return -1;
+  DISN_CUDA_OK(cudaMemcpyAsync(c->d_idx.as<int32_t>(), idx, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  DISN_CUDA_OK(cudaMemcpyAsync(c->d_tm.as<float>(), trans_mat, 12 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  if (eval_indexed(c, image, R, c->d_tm.as<float>(), c->d_idx.as<int32_t>(), n, c->d_out.as<float>())) return -1;
+  DISN_CUDA_OK(cudaMemcpyAsync(out, c->d_out.as<float>(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
+  return check_status(c);
+}
+
+int disn_eval_grid_adaptive(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t image, int32_t sdf_res,
+                            float iso, double band, float** grid_dev, int64_t* level_counts, int32_t* n_levels) {
+  DISN_REQUIRE(c && sdf_params && trans_mat && grid_dev && level_counts && n_levels, "null argument");
+  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(image >= 0 && image < c->enc_B, "image outside the encoded batch");
+  DISN_REQUIRE(sdf_res >= 1 && (int64_t)(sdf_res + 1) * (sdf_res + 1) * (sdf_res + 1) <= INT32_MAX,
+               "eval_grid_adaptive: 1 <= sdf_res and (sdf_res+1)^3 < 2^31");
+  DISN_REQUIRE(std::isfinite(iso), "eval_grid_adaptive: iso must be finite");
+  DISN_REQUIRE(!std::isnan(band) && band >= 0.0, "eval_grid_adaptive: band must be >= 0 (+inf evaluates every point)");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  if (grid_axes(c, sdf_params, 1, sdf_res + 1)) return -1;
+  DISN_CUDA_OK(cudaMemcpyAsync(c->d_tm.as<float>(), trans_mat, 12 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  if (adaptive_run(c, nullptr, image, c->d_tm.as<float>(), sdf_res, sdf_params, iso, band, level_counts, n_levels))
+    return -1;
+  DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
+  if (const int rc = check_status(c)) return rc;
+  *grid_dev = c->ad_grid.as<float>();
+  return 0;
+}
+
 // ---- cross-process device buffers (multi-GPU gather without a collective) -------------------------------------------
 // Rank 0 allocates the whole-grid buffer and exports a CUDA IPC handle; the other ranks (one process per GPU) open it and
 // pass `ptr + slab offset` as the DISN_DEVICE_PTR output of disn_eval_grid, so the kernel's epilogue stores every
@@ -653,3 +694,37 @@ int disn_fetch(disn_ctx* c, const void* dev, void* host, int64_t bytes) {
 }  // extern "C"
 
 void disn::axis_table(double start, double stop, int num, float* out) { linspace_f32(start, stop, num, out); }
+
+// axis tables (host float64 linspace -> float32): B*3*R floats, re-uploaded only when the boxes / resolution change (keeps
+// repeated calls free of host syncs)
+int disn::grid_axes(disn_ctx* c, const double* sdf_params, int B, int R) {
+  const size_t axes_bytes = (size_t)8 * 3 * R * sizeof(float);
+  if (axes_bytes > c->d_axes.bytes()) c->axes_key.clear();   // a new allocation holds no tables yet
+  if (c->d_axes.ensure(axes_bytes)) return -1;
+  std::vector<double> key(sdf_params, sdf_params + (size_t)B * 6);
+  key.push_back((double)R);
+  if (key != c->axes_key) {
+    std::vector<float> axes((size_t)B * 3 * R);
+    for (int b = 0; b < B; ++b)
+      for (int a = 0; a < 3; ++a)
+        linspace_f32(sdf_params[b * 6 + a], sdf_params[b * 6 + 3 + a], R, &axes[((size_t)b * 3 + a) * R]);
+    DISN_CUDA_OK(cudaMemcpyAsync(c->d_axes.as<float>(), axes.data(), axes.size() * sizeof(float), cudaMemcpyHostToDevice,
+                                 c->stream));
+    DISN_CUDA_OK(cudaStreamSynchronize(c->stream));   // `axes` is a stack-owned staging buffer
+    c->axes_key = key;
+  }
+  return 0;
+}
+
+// One image of the encoded batch as a batch of one: its gbias / pmap rows, its matrix and the first axis tables.
+int disn::eval_indexed(disn_ctx* c, int image, int R, const float* d_tm, const int32_t* idx, int64_t n, float* out) {
+  if (n == 0) return 0;
+  PointJob job{};
+  job.B = 1; job.N = n; job.R = R; job.z0 = 0; job.idx = idx; job.axes = c->d_axes.as<float>();
+  job.gbias = c->gbias.as<float>() + (int64_t)image * kHidden;
+  job.pmap = c->pmap.as<float>() + (int64_t)image * c->cfg.img_h * c->cfg.img_w * kHidden;
+  job.trans_mat = d_tm;
+  job.out_pred = out;
+  job.out_div = c->cfg.sdf_weight;
+  return run_point_job(c, job);
+}

@@ -156,6 +156,8 @@ struct PointJob {
   const float* axes;      // grid mode: [B,3,R] float32 linspace tables (x,y,z)
   int32_t R;              // grid mode: points per axis
   int32_t z0;             // grid mode: first z plane
+  const int32_t* idx;     // grid mode: point n is grid point idx[n] = (z*R + y)*R + x (z0 = 0), or nullptr: point n is
+                          // z0*R^2 + n (the dense slab)
   int64_t N;              // points per image in this call
   int32_t B;
   // per-image encoder products
@@ -179,6 +181,18 @@ struct PointJob {
 };
 
 constexpr int DISN_STATUS_FP16_OVERFLOW = 1;   // DISN_PREC_F16F8: an activation exceeded fp16's range
+constexpr int DISN_STATUS_BAD_INDEX = 2;       // grid mode with idx: an index outside [0, R^3) (evaluated as point 0)
+
+// linear grid index of point n of a grid-mode job (see PointJob::idx)
+__device__ __forceinline__ int64_t grid_index(const PointJob& job, int64_t n) {
+  if (!job.idx) return n;
+  const int64_t i = job.idx[n];
+  if (i < 0 || i >= (int64_t)job.R * job.R * job.R) {
+    if (job.status) atomicOr(job.status, DISN_STATUS_BAD_INDEX);
+    return 0;
+  }
+  return i;
+}
 
 }  // namespace disn
 
@@ -256,6 +270,14 @@ struct disn_ctx {
   int64_t smp_n[4] = {};
   // device-resident SDF grid of disn_eval_grid_resident and host staging for the marching-cubes input
   disn::DevBuffer d_grid;
+  disn::DevBuffer d_idx;        // host-index staging of disn_eval_grid_indexed
+  // coarse-to-fine grid (adaptive.cu): the filled grid, one byte per point (1 = evaluated), the block states of every
+  // level, the per-level index list and its values, compaction counts and scan scratch, host-field staging, the
+  // pinned level total and the phase events; ad_R / ad_levels describe the last call
+  disn::DevBuffer ad_grid, ad_mark, ad_state, ad_list, ad_vals, ad_chunk, ad_sums, ad_field;
+  disn::PinnedBuffer ad_host;
+  cudaEvent_t ad_ev[7] = {};
+  int32_t ad_R = 0, ad_levels = 0;
   disn::DevBuffer d_mc_in;
   // nn_distance / cam scratch (persistent, grows)
   disn::DevBuffer nn_scratch;
@@ -314,4 +336,13 @@ int band_gather(disn_ctx* c, const float* axes, const int64_t* choices, const in
 int sdf_strided(disn_ctx* c, const float* sdf, int32_t R, int32_t reduce, bool device_ptr, float* out);
 // api.cu: numpy.linspace(start, stop, num) in float64 cast to float32 (the grid coordinates of eval_grid and mesh_sdf)
 void axis_table(double start, double stop, int num, float* out);
+// api.cu: the float32 axis tables of B boxes in c->d_axes (uploaded only when boxes or R change)
+int grid_axes(disn_ctx* c, const double* sdf_params, int B, int R);
+// api.cu: grid points idx[0..n) (device) of encoded image `image` -> out[0..n) (device) = pred/sdf_weight; the axis tables
+// of that image's box must be in c->d_axes (grid_axes with B = 1); d_tm: the image's [4,3] matrix on the device
+int eval_indexed(disn_ctx* c, int image, int R, const float* d_tm, const int32_t* idx, int64_t n, float* out);
+// adaptive.cu: coarse-to-fine grid of one image; values come from `field` (device [R,R,R]) when it is non-null, else from
+// the network (eval_indexed, with d_tm and the axis tables as above).  The filled grid stays in c->ad_grid.
+int adaptive_run(disn_ctx* c, const float* field, int image, const float* d_tm, int32_t res, const double* sdf_params,
+                 float iso, double band, int64_t* level_counts, int32_t* n_levels);
 }  // namespace disn

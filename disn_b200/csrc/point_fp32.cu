@@ -223,8 +223,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) point_fp32_kernel(PointJob job, i
           } else { xr = x; yr = y; zr = z; }
         } else {
           const int R = job.R;
-          int ix = (int)(n % R);
-          int64_t t = n / R;
+          const int64_t m = grid_index(job, n);
+          int ix = (int)(m % R);
+          int64_t t = m / R;
           int iy = (int)(t % R);
           int iz = (int)(t / R) + job.z0;
           const float* ax = job.axes + (int64_t)b * 3 * R;

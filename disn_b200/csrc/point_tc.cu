@@ -77,7 +77,9 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// query point n of image b: (x, y, z) is projected, (xr, yr, zr) feeds the MLP; zeros past the end
+// query point n of image b: (x, y, z) is projected, (xr, yr, zr) feeds the MLP; zeros past the end.  kIdx: grid point
+// job.idx[n] (a separate instantiation, so the dense kernel is the same code as without the indexed path)
+template <bool kIdx>
 __device__ __forceinline__ void point_of(const PointJob& job, int b, int64_t n, float& x, float& y, float& z, float& xr,
                                          float& yr, float& zr) {
   x = y = z = xr = yr = zr = 0.f;
@@ -91,8 +93,9 @@ __device__ __forceinline__ void point_of(const PointJob& job, int b, int64_t n, 
     } else { xr = x; yr = y; zr = z; }
   } else {
     const int R = job.R;
-    const int ix = (int)(n % R);
-    const int64_t tt = n / R;
+    const int64_t m = kIdx ? grid_index(job, n) : n;
+    const int ix = (int)(m % R);
+    const int64_t tt = m / R;
     const int iy = (int)(tt % R);
     const int iz = (int)(tt / R) + job.z0;
     const float* ax = job.axes + (int64_t)b * 3 * R;
@@ -109,6 +112,7 @@ __device__ __forceinline__ void project(const PointJob& job, int b, float x, flo
   v = fminf(job.clamp_max, fmaxf(0.f, q1 / q2));
 }
 // bilinear taps of point n into the projected feature map (element offsets, -1 = outside; weights 0 there)
+template <bool kIdx>
 __device__ __forceinline__ void taps_of(const PointJob& job, int b, int64_t n, int (&off)[4], float (&wg)[4]) {
 #pragma unroll
   for (int k = 0; k < 4; ++k) { off[k] = -1; wg[k] = 0.f; }
@@ -119,7 +123,7 @@ __device__ __forceinline__ void taps_of(const PointJob& job, int b, int64_t n, i
     return;
   }
   float x, y, z, xr, yr, zr, u, v;
-  point_of(job, b, n, x, y, z, xr, yr, zr);
+  point_of<kIdx>(job, b, n, x, y, z, xr, yr, zr);
   project(job, b, x, y, z, u, v);
   const int Wm = job.img_w, Hm = job.img_h;
   if (u > -1.f && v > -1.f && u < (float)Wm && v < (float)Hm) {
@@ -167,7 +171,7 @@ __device__ __forceinline__ void store_pair(uint8_t* xs, int row, int k, float a,
 //             a.(w - h(w)) ("second") for tensor layer l = 0..3 (fold1/conv2, fold1/conv3, fold2/conv1, fold2/conv2).
 //             0xFF = every correction; the shipped mask is CORR_DEFAULT.
 // the consumers hold two 64-register accumulators (plus the 32-register correction accumulator of MODE_F16F8)
-template <int kMode, int kCorr>
+template <int kMode, int kCorr, bool kIdx>
 __global__ void __launch_bounds__(NCONS, 1)
 point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint8_t* __restrict__ wpk,
                  int64_t tiles_per_img) {
@@ -222,7 +226,7 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
         const int p = tid >> 2, f0 = (tid & 3) * 16;
         const int64_t n = n0 + p;
         float x, y, z, xr, yr, zr;
-        point_of(job, b, n, x, y, z, xr, yr, zr);
+        point_of<kIdx>(job, b, n, x, y, z, xr, yr, zr);
         if (sx == 0 && (tid & 3) == 0 && job.out_uv && n < job.N) {
           float u, v;
           project(job, b, x, y, z, u, v);
@@ -320,8 +324,8 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
           int off[2][4];
           float wg[2][4];
           if (gather) {
-            taps_of(job, b, n0 + r0, off[0], wg[0]);
-            taps_of(job, b, n0 + r0 + 8, off[1], wg[1]);
+            taps_of<kIdx>(job, b, n0 + r0, off[0], wg[0]);
+            taps_of<kIdx>(job, b, n0 + r0 + 8, off[1], wg[1]);
           }
           const float* pm = job.pfeat ? job.pfeat : job.pmap + (int64_t)b * job.img_h * job.img_w * kHidden;
           const int sb = layer == 0 ? SB_B2 : (layer == 1 ? SB_B3 : SB_B4);
@@ -404,18 +408,18 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
   }
 }
 
-template <int kMode, int kCorr>
+template <int kMode, int kCorr, bool kIdx>
 int launch_var(disn_ctx* c, const PointJob& job, const SmallParams& sp, const void* wpk, int grid, int smem,
                int64_t tiles_per_img) {
   // the attribute belongs to (function, device): set per context, not per process (a second engine on another device
   // in the same process would otherwise launch with the 48 KB default)
-  auto key = (const void*)point_tc_kernel<kMode, kCorr>;
+  auto key = (const void*)point_tc_kernel<kMode, kCorr, kIdx>;
   if (!c->attr_done.count(key)) {
-    DISN_CUDA_OK(cudaFuncSetAttribute(point_tc_kernel<kMode, kCorr>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    DISN_CUDA_OK(cudaFuncSetAttribute(point_tc_kernel<kMode, kCorr, kIdx>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     c->attr_done.insert(key);
   }
-  point_tc_kernel<kMode, kCorr><<<grid, NCONS, smem, c->stream>>>(job, sp, reinterpret_cast<const uint8_t*>(wpk),
-                                                                     tiles_per_img);
+  point_tc_kernel<kMode, kCorr, kIdx><<<grid, NCONS, smem, c->stream>>>(job, sp, reinterpret_cast<const uint8_t*>(wpk),
+                                                                           tiles_per_img);
   return 0;
 }
 
@@ -542,11 +546,20 @@ int launch_point_tc(disn_ctx* c, const PointJob& job_in) {
   int corr = CORR_DEFAULT;
   if (const char* e = getenv("DISN_TC_CORR")) corr = (int)strtol(e, nullptr, 0);      // A/B: 0xFF = every correction
   int rc = -2;
-  if (!f8) rc = launch_var<MODE_BF16X3, 0xFF>(c, job, sp, wpk, grid, smem, tiles_per_img);
-  else {
+  const bool idx = job.idx != nullptr;
+  if (!f8) {
+    rc = idx ? launch_var<MODE_BF16X3, 0xFF, true>(c, job, sp, wpk, grid, smem, tiles_per_img)
+             : launch_var<MODE_BF16X3, 0xFF, false>(c, job, sp, wpk, grid, smem, tiles_per_img);
+  } else {
     switch (corr) {
-      case 0xFF: rc = launch_var<MODE_F16F8, 0xFF>(c, job, sp, wpk, grid, smem, tiles_per_img); break;
-      case 0xDF: rc = launch_var<MODE_F16F8, 0xDF>(c, job, sp, wpk, grid, smem, tiles_per_img); break;
+      case 0xFF:
+        rc = idx ? launch_var<MODE_F16F8, 0xFF, true>(c, job, sp, wpk, grid, smem, tiles_per_img)
+                 : launch_var<MODE_F16F8, 0xFF, false>(c, job, sp, wpk, grid, smem, tiles_per_img);
+        break;
+      case 0xDF:
+        rc = idx ? launch_var<MODE_F16F8, 0xDF, true>(c, job, sp, wpk, grid, smem, tiles_per_img)
+                 : launch_var<MODE_F16F8, 0xDF, false>(c, job, sp, wpk, grid, smem, tiles_per_img);
+        break;
       default: DISN_REQUIRE(false, "DISN_TC_CORR: only 0xFF (all corrections) and 0xDF (default) are built");
     }
   }

@@ -485,6 +485,43 @@ class Engine:
                                                t.ctypes.data_as(C.c_void_p), sp.shape[0], sdf_res, C.byref(out)))
         return int(out.value)
 
+    def eval_grid_indexed(self, sdf_params, trans_mat, sdf_res: int, idx, image: int = 0):
+        """Grid points idx (linear (z*R + y)*R + x, any order) of encoded image `image` -> float32 [n], bitwise the
+        values eval_grid gives at those points.  sdf_params [6] and trans_mat [4,3] belong to that image."""
+        sp = np.ascontiguousarray(sdf_params, dtype=np.float64).reshape(6)
+        t = _f32(trans_mat).reshape(4, 3)
+        ix = np.ascontiguousarray(idx, dtype=np.int64).reshape(-1)
+        if ix.size and (ix.min() < 0 or ix.max() >= 2 ** 31):
+            raise ValueError("grid indices must lie in [0, 2^31)")
+        ix = ix.astype(np.int32)
+        out = np.empty(ix.size, np.float32)
+        check(self.lib.disn_eval_grid_indexed(self._h, sp.ctypes.data_as(C.POINTER(C.c_double)), t.ctypes.data_as(C.c_void_p),
+                                              image, sdf_res, ix.ctypes.data_as(C.c_void_p), ix.size,
+                                              out.ctypes.data_as(C.c_void_p), 0))
+        return out
+
+    def eval_grid_indexed_device(self, sdf_params, trans_mat_ptr: int, sdf_res: int, idx_ptr: int, n: int, out_ptr: int,
+                                 image: int = 0):
+        """Device-pointer, asynchronous variant: int32 indices at idx_ptr, float32 results at out_ptr."""
+        sp = np.ascontiguousarray(sdf_params, dtype=np.float64).reshape(6)
+        check(self.lib.disn_eval_grid_indexed(self._h, sp.ctypes.data_as(C.POINTER(C.c_double)), C.c_void_p(trans_mat_ptr),
+                                              image, sdf_res, C.c_void_p(idx_ptr), n, C.c_void_p(out_ptr), DISN_DEVICE_PTR))
+
+    def eval_grid_adaptive(self, sdf_params, trans_mat, sdf_res: int, iso: float = 0.0, band: float = 1.0, image: int = 0):
+        """Coarse-to-fine [R,R,R] grid of encoded image `image` (DESIGN.md §4.9), left in the context's HBM buffer ->
+        (device address, points evaluated by the coarse lattice and by each level).  The network runs only in blocks that
+        straddle iso or lie within band * (s/2) * |h| of it; the other points are interpolated.  band = inf is the dense
+        grid."""
+        sp = np.ascontiguousarray(sdf_params, dtype=np.float64).reshape(6)
+        t = _f32(trans_mat).reshape(4, 3)
+        out = C.c_void_p()
+        counts = np.zeros(5, np.int64)
+        nl = C.c_int32(0)
+        check(self.lib.disn_eval_grid_adaptive(self._h, sp.ctypes.data_as(C.POINTER(C.c_double)), t.ctypes.data_as(C.c_void_p),
+                                               image, sdf_res, float(iso), float(band), C.byref(out),
+                                               counts.ctypes.data_as(C.c_void_p), C.byref(nl)))
+        return int(out.value), [int(v) for v in counts[:nl.value]]
+
     def fetch(self, dev_ptr: int, shape, dtype=np.float32) -> np.ndarray:
         out = np.empty(shape, dtype=dtype)
         check(self.lib.disn_fetch(self._h, C.c_void_p(dev_ptr), out.ctypes.data_as(C.c_void_p), out.nbytes))

@@ -132,6 +132,26 @@ int disn_marching_cubes(disn_ctx* ctx, const float* sdf, int32_t R, const double
  * a synchronous device->host copy on the context's stream (e.g. to keep the .dist artefact). */
 int disn_eval_grid_resident(disn_ctx* ctx, const double* sdf_params, const float* trans_mat, int32_t B,
                             int32_t sdf_res, float** out_dev);
+
+/* Indexed grid: the grid points idx[0..n) (int32 linear indices (z*R + y)*R + x, any order, R = sdf_res+1, R^3 < 2^31) of
+ * encoded image `image`, with sdf_params host double[6] (that image's box) and trans_mat [4,3] -> out[n] = pred/sdf_weight.
+ * Every value is bitwise the value disn_eval_grid produces at that point, in every precision.  idx, trans_mat and out are
+ * host pointers (indices checked on the host), or device pointers with DISN_DEVICE_PTR (asynchronous; an index outside
+ * the grid is reported by the next synchronising call).  The DISN_PREC_F16F8 overflow status works as for disn_eval_grid. */
+int disn_eval_grid_indexed(disn_ctx* ctx, const double* sdf_params, const float* trans_mat, int32_t image, int32_t sdf_res,
+                           const int32_t* idx, int64_t n, float* out, uint32_t flags);
+
+/* Coarse-to-fine grid of encoded image `image` (DESIGN.md 4.9): the network is evaluated on the stride-s0 lattice (s0 =
+ * the largest power of two <= 16 dividing sdf_res) and then only inside blocks whose corners straddle iso or lie within
+ * band * (s/2) * |h| of it; every other point is the trilinear interpolation of an inactive block's corners.  The complete
+ * [R,R,R] grid stays in HBM (*grid_dev, valid until the next call; mesh it with disn_mc_run and DISN_DEVICE_PTR).  For a
+ * 1-Lipschitz field and band >= 1 its marching-cubes mesh equals the dense grid's; band = +inf evaluates every point.
+ * sdf_params host double[6], trans_mat host [4,3]; level_counts (at least 5 entries) receives the points evaluated by
+ * the coarse lattice and by each level, *n_levels their number.  iso must be finite and band >= 0.  Synchronises once
+ * per level. */
+int disn_eval_grid_adaptive(disn_ctx* ctx, const double* sdf_params, const float* trans_mat, int32_t image,
+                            int32_t sdf_res, float iso, double band, float** grid_dev, int64_t* level_counts,
+                            int32_t* n_levels);
 int disn_mc_run(disn_ctx* ctx, const float* sdf, int32_t R, const double* bbox, float iso, uint32_t flags,
                 int64_t* n_verts, int64_t* n_faces);
 int disn_mc_fetch(disn_ctx* ctx, float* verts, int32_t* faces);

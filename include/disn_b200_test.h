@@ -26,6 +26,17 @@ int disn_tc_stream_probe(int device);
 /* Diagnostic: prints the issue cost (cycles) of the mbarrier / wgmma synchronisation instructions of the consumers. */
 int disn_tc_op_probe(int device);
 
+/* Diagnostics of the coarse-to-fine grid (disn_eval_grid_adaptive):
+ *   disn_adaptive_mask: points [first, first + n) of the last call's evaluated-point mask -> out uint8[n] (1 = evaluated);
+ *   disn_adaptive_from_field: the same refinement with values read from field [R,R,R] (host, or device with
+ *     DISN_DEVICE_PTR) instead of the network; sdf_params[6] gives the box (the spacing of the band);
+ *   disn_adaptive_phase_ms: device-event milliseconds of the last call's phases -- coarse lattice (or the dense grid),
+ *     each level, fill -- into ms (at least 6 entries), *n their number. */
+int disn_adaptive_mask(disn_ctx* ctx, int64_t first, int64_t n, uint8_t* out);
+int disn_adaptive_from_field(disn_ctx* ctx, const float* field, int32_t sdf_res, const double* sdf_params, float iso,
+                             double band, uint32_t flags, float** grid_dev, int64_t* level_counts, int32_t* n_levels);
+int disn_adaptive_phase_ms(disn_ctx* ctx, float* ms, int32_t* n);
+
 #ifdef __cplusplus
 }
 #endif
