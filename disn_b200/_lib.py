@@ -56,6 +56,9 @@ EXPORTS = {
                                          C.c_int64, C.c_void_p, C.c_uint32]),
     "disn_eval_grid_adaptive": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_int32, C.c_int32, C.c_float,
                                           C.c_double, C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_int32)]),
+    "disn_mesh_grid_adaptive": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_int32, C.c_int32, C.c_float,
+                                          C.c_double, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                          C.POINTER(C.c_int64)]),
     "disn_mc_run": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_float, C.c_uint32,
                               C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "disn_mc_fetch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -101,6 +104,12 @@ TEST_EXPORTS = {
     "disn_adaptive_from_field": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_float, C.c_double,
                                            C.c_uint32, C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_int32)]),
     "disn_adaptive_phase_ms": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]),
+    "disn_mesh_adaptive_from_field": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_float,
+                                                C.c_double, C.c_uint32, C.c_void_p, C.POINTER(C.c_int32),
+                                                C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "disn_mesh_adaptive_phase_ms": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "disn_mesh_adaptive_bytes": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
+    "disn_mesh_adaptive_edges": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
 }
 
 _lib = None

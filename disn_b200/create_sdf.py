@@ -104,6 +104,13 @@ def create(weights, batches, device=0):
         sess.close()
 
 
+# FLAGS.adaptive without keep_dist meshes through Engine.mesh_grid_adaptive from this sdf_res on: the first resolution the
+# dense adaptive grid plus marching cubes cannot run (marching cubes needs 3 (sdf_res+1)^3 < 2^32, so sdf_res <= 1126).
+# Wherever that path runs it is faster (H100 80GB HBM3, 700 W, tools/adaptive_mesh_bench.py, BASELINE.md §8: 2.4 s
+# against 8.3 s at 1025^3 on the median iso, 0.48 s against 2.9 s on the 0.95 quantile).
+SURFACE_MESH_MIN_RES = 1127
+
+
 def build_grid_points(sdf_params_b):
     """test/create_sdf.py:246-255 -- host float64 linspace grid, (x,y,z) float32, x fastest."""
     x_ = np.linspace(sdf_params_b[0], sdf_params_b[3], num=RESOLUTION)
@@ -129,9 +136,11 @@ def test_one_epoch(sess, ops, batches):
     No .dist round trip through the file system; FLAGS.keep_dist=True also writes the reference's .dist artefact.
     FLAGS.clean_smallparts=True runs the reference's postprocessing/clean_smallparts.py step on each mesh while it is
     still in HBM (thresholds FLAGS.clean_dist_thresh / clean_num_thresh, default 0.5 / 0.3).
-    FLAGS.adaptive=True (default False) replaces the batch's dense grid with one coarse-to-fine grid per image
-    (Engine.eval_grid_adaptive, band FLAGS.adaptive_band, default 1.0): the network runs only near the surface; output
-    names, cleaning, keep_dist and the OBJ writer are unchanged.
+    FLAGS.adaptive=True (default False) replaces the batch's dense grid with coarse-to-fine evaluation per image (band
+    FLAGS.adaptive_band, default 1.0): the network runs only near the surface.  From sdf_res SURFACE_MESH_MIN_RES on and
+    without keep_dist no grid is built: Engine.mesh_grid_adaptive meshes from the surface blocks alone (DESIGN.md §4.10,
+    the same mesh bit for bit); otherwise Engine.eval_grid_adaptive builds the grid.  Output names, cleaning and the OBJ
+    writer are unchanged.
     The reference's literal loop (host grid, SPLIT_SIZE chunks through sess.run, reassembly, /SDF_WEIGHT) is kept as a
     verification aid in tests/reference_loop.py."""
     log_string(str(datetime.now()))
@@ -150,13 +159,27 @@ def test_one_epoch(sess, ops, batches):
                     print("{}/{}, submit create_obj {}, {}, {}".format(batch_idx, "?", batch_data["cat_id"][b],
                                                                        batch_data["obj_nm"][b], batch_data["view_id"][b]))
                     path = obj_path(RESULT_OBJ_PATH, batch_data["cat_id"][b], batch_data["obj_nm"][b], batch_data["view_id"][b])
-                    if adaptive:        # coarse-to-fine grid of this image (DESIGN.md §4.9), meshed before the next one
+                    keep_dist = getattr(FLAGS, "keep_dist", False)
+                    band = float(getattr(FLAGS, "adaptive_band", 1.0))
+                    if adaptive and not keep_dist and FLAGS.sdf_res >= SURFACE_MESH_MIN_RES:
+                        # no grid needed: mesh from the surface blocks (DESIGN.md §4.10)
+                        sess.engine.mesh_grid_adaptive(
+                            np.asarray(batch_data["sdf_params"], np.float64)[b], np.asarray(batch_data["trans_mat"])[b],
+                            FLAGS.sdf_res, iso=float(FLAGS.iso), band=band, image=b, fetch=False)
+                        dev = None
+                    elif adaptive:      # coarse-to-fine grid of this image (DESIGN.md §4.9), meshed before the next one
                         dev, _ = sess.engine.eval_grid_adaptive(
                             np.asarray(batch_data["sdf_params"], np.float64)[b], np.asarray(batch_data["trans_mat"])[b],
-                            FLAGS.sdf_res, iso=float(FLAGS.iso), band=float(getattr(FLAGS, "adaptive_band", 1.0)), image=b)
+                            FLAGS.sdf_res, iso=float(FLAGS.iso), band=band, image=b)
                     else:
                         dev = grid_ptr + b * R * R * R * 4
-                    if getattr(FLAGS, "clean_smallparts", False):
+                    if dev is None:
+                        if getattr(FLAGS, "clean_smallparts", False):
+                            verts, faces = sess.engine.clean_mesh(getattr(FLAGS, "clean_dist_thresh", 0.5),
+                                                                  getattr(FLAGS, "clean_num_thresh", 0.3))
+                        else:
+                            verts, faces = sess.engine.fetch_mesh()
+                    elif getattr(FLAGS, "clean_smallparts", False):
                         # postprocessing/clean_smallparts.py on the resident mesh before it leaves HBM
                         sess.engine.marching_cubes(None, batch_data["sdf_params"][b], float(FLAGS.iso), device_ptr=dev,
                                                    R=R, fetch=False)
@@ -165,7 +188,7 @@ def test_one_epoch(sess, ops, batches):
                     else:
                         verts, faces = sess.engine.marching_cubes(None, batch_data["sdf_params"][b], float(FLAGS.iso),
                                                                   device_ptr=dev, R=R)
-                    if getattr(FLAGS, "keep_dist", False):
+                    if keep_dist:
                         to_binary(R - 1, batch_data["sdf_params"][b], sess.engine.fetch(dev, (R, R, R)), path[:-4] + ".dist")
                     futures.append(executor.submit(_write_and_return, path, verts, faces))
         for f in futures:

@@ -19,6 +19,7 @@
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
 
+#include "adaptive_common.cuh"
 #include "common.cuh"
 
 namespace disn {
@@ -27,7 +28,6 @@ namespace {
 constexpr int AD_THREADS = 256;
 constexpr int AD_ITEMS = 8;
 constexpr int AD_CHUNK = AD_THREADS * AD_ITEMS;   // mark bytes per compaction block
-constexpr int AD_MAX_LEVELS = 4;                   // s0 <= 16: levels 16, 8, 4, 2
 
 inline unsigned blocks_of(int64_t n) { return (unsigned)((n + AD_THREADS - 1) / AD_THREADS); }
 
@@ -73,15 +73,10 @@ __global__ void __launch_bounds__(AD_THREADS) classify_kernel(const float* __res
   }
   const int64_t o = ((int64_t)bz * s * R + (int64_t)by * s) * R + (int64_t)bx * s;
   const int64_t dx = s, dy = (int64_t)s * R, dz = (int64_t)s * R * R;
-  int below = 0;
-  bool near = false;
+  float v[8];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const float v = grid[o + ((k & 1) ? dx : 0) + ((k & 2) ? dy : 0) + ((k & 4) ? dz : 0)];
-    below += (v < iso) ? 1 : 0;
-    near |= fabsf(__fsub_rn(v, iso)) <= tau;
-  }
-  const bool active = (below != 0 && below != 8) || near;
+  for (int k = 0; k < 8; ++k) v[k] = grid[o + ((k & 1) ? dx : 0) + ((k & 2) ? dy : 0) + ((k & 4) ? dz : 0)];
+  const bool active = block_active(v, iso, tau);
   st[b] = active ? 2 : 1;
   if (!active) return;
   const int h = s >> 1;
@@ -129,20 +124,6 @@ __global__ void __launch_bounds__(AD_THREADS) compact_kernel(uint8_t* __restrict
     }
 }
 
-__device__ __forceinline__ float lerp_rn(float t, float a, float b) {
-  return __fadd_rn(__fmul_rn(__fsub_rn(1.f, t), a), __fmul_rn(t, b));
-}
-
-// candidate block origins (in blocks) of coordinate c at block size s: the block starting at or below c, then the block
-// ending at c; returns how many are valid
-__device__ __forceinline__ int block_candidates(int c, int s, int nb, int (&q)[2]) {
-  int k = 0;
-  const int q0 = c / s;
-  if (q0 < nb) q[k++] = q0;
-  if (c % s == 0 && q0 >= 1) q[k++] = q0 - 1;
-  return k;
-}
-
 __global__ void __launch_bounds__(AD_THREADS) fill_kernel(float* __restrict__ grid, const uint8_t* __restrict__ mark,
                                                           const uint8_t* __restrict__ st, int R, Levels lv) {
   const int64_t i = (int64_t)blockIdx.x * AD_THREADS + threadIdx.x;
@@ -161,15 +142,10 @@ __global__ void __launch_bounds__(AD_THREADS) fill_kernel(float* __restrict__ gr
           const float tx = (float)(x - ox) * inv, ty = (float)(y - oy) * inv, tz = (float)(z - oz) * inv;
           const int64_t o = ((int64_t)oz * R + oy) * R + ox;
           const int64_t sy = (int64_t)s * R, sz = (int64_t)s * R * R;
-          float cz[2];
+          float v[8];
 #pragma unroll
-          for (int kz = 0; kz < 2; ++kz) {
-            const int64_t p = o + kz * sz;
-            const float c0 = lerp_rn(tx, grid[p], grid[p + s]);
-            const float c1 = lerp_rn(tx, grid[p + sy], grid[p + sy + s]);
-            cz[kz] = lerp_rn(ty, c0, c1);
-          }
-          grid[i] = lerp_rn(tz, cz[0], cz[1]);
+          for (int k = 0; k < 8; ++k) v[k] = grid[o + ((k & 1) ? s : 0) + ((k & 2) ? sy : 0) + ((k & 4) ? sz : 0)];
+          grid[i] = trilinear(v, tx, ty, tz);
           return;
         }
   }
@@ -197,8 +173,7 @@ int adaptive_run(disn_ctx* c, const float* field, int image, const float* d_tm, 
                  float iso, double band, int64_t* level_counts, int32_t* n_levels) {
   const int R = res + 1;
   const int64_t n = (int64_t)R * R * R;
-  int s0 = 16;
-  while (s0 > 1 && res % s0) s0 >>= 1;
+  const int s0 = coarse_stride(res);
   Levels lv{};
   int64_t states = 0;
   for (int s = s0; s >= 2; s >>= 1, ++lv.n) {
@@ -248,13 +223,10 @@ int adaptive_run(disn_ctx* c, const float* field, int image, const float* d_tm, 
   level_counts[0] = M * M * M;
   DISN_CUDA_OK(cudaEventRecord(c->ad_ev[1], st));
 
-  const double hx = (sdf_params[3] - sdf_params[0]) / res, hy = (sdf_params[4] - sdf_params[1]) / res,
-               hz = (sdf_params[5] - sdf_params[2]) / res;
-  const double diag = std::sqrt(hx * hx + hy * hy + hz * hz);
   uint32_t* h_total = c->ad_host.as<uint32_t>();
   for (int l = 0; l < lv.n; ++l) {
     const int s = lv.s[l], nb = lv.nb[l];
-    const float tau = (float)(band * (s / 2) * diag);
+    const float tau = level_tau(band, s, sdf_params, res);
     const int64_t nblk = (int64_t)nb * nb * nb;
     classify_kernel<<<blocks_of(nblk), AD_THREADS, 0, st>>>(grid, R, s, nb, l ? state + lv.off[l - 1] : nullptr,
                                                             state + lv.off[l], mark, iso, tau);

@@ -5,6 +5,7 @@
 #include <memory>
 #include <vector>
 
+#include "adaptive_common.cuh"
 #include "common.cuh"
 
 namespace disn {
@@ -19,6 +20,8 @@ disn_ctx::~disn_ctx() {
   for (cudaEvent_t e : sdf_ev)
     if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ad_ev)
+    if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : am_ev)
     if (e) cudaEventDestroy(e);
   if (own_stream && stream) cudaStreamDestroy(stream);
 }
@@ -645,6 +648,59 @@ int disn_eval_grid_adaptive(disn_ctx* c, const double* sdf_params, const float* 
   if (const int rc = check_status(c)) return rc;
   *grid_dev = c->ad_grid.as<float>();
   return 0;
+}
+
+}  // extern "C"
+
+// End of a call that builds the resident mesh: on failure the resident mesh is emptied (it may be half replaced or built
+// from invalid values), and the resident counts are reported either way, so a caller's view of the slot always matches
+// what disn_mc_fetch copies.
+int disn::finish_mesh_call(disn_ctx* c, int rc, int64_t* n_verts, int64_t* n_faces) {
+  if (rc) {
+    c->mc_nv = c->mc_nf = 0;
+    c->am_nv = -1;
+  }
+  if (n_verts) *n_verts = c->mc_nv;
+  if (n_faces) *n_faces = c->mc_nf;
+  return rc;
+}
+
+extern "C" {
+
+int disn_mesh_grid_adaptive(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t image, int32_t sdf_res,
+                            float iso, double band, int64_t* level_counts, int32_t* n_levels, int64_t* n_verts,
+                            int64_t* n_faces) {
+  DISN_REQUIRE(c && sdf_params && trans_mat && level_counts && n_levels, "null argument");
+  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(image >= 0 && image < c->enc_B, "image outside the encoded batch");
+  DISN_REQUIRE(sdf_res >= 1 && sdf_res <= 2048, "mesh_grid_adaptive: 1 <= sdf_res <= 2048");
+  DISN_REQUIRE(std::isfinite(iso), "mesh_grid_adaptive: iso must be finite");
+  DISN_REQUIRE(!std::isnan(band) && band >= 0.0, "mesh_grid_adaptive: band must be >= 0 (+inf evaluates every point)");
+  const int64_t R = sdf_res + 1;
+  DISN_REQUIRE(coarse_stride(sdf_res) > 1 || (R * R * R <= INT32_MAX && 3 * R * R * R < ((int64_t)1 << 32)),
+               "mesh_grid_adaptive: an odd sdf_res (no power of two divides it) evaluates the dense grid, which needs "
+               "(sdf_res+1)^3 < 2^31 and 3 (sdf_res+1)^3 < 2^32 (sdf_res <= 1125)");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  int rc = grid_axes(c, sdf_params, 1, sdf_res + 1);
+  if (!rc && cudaMemcpyAsync(c->d_tm.as<float>(), trans_mat, 12 * sizeof(float), cudaMemcpyHostToDevice, c->stream)) {
+    set_error("mesh_grid_adaptive: trans_mat upload failed");
+    rc = -1;
+  }
+  if (!rc && coarse_stride(sdf_res) == 1) {     // the dense grid, as disn_eval_grid_adaptive evaluates it, then MC
+    c->am_nv = -1;                              // the mesher's diagnostics describe no call until its next one
+    c->am_edges_sorted = nullptr;
+    rc = adaptive_run(c, nullptr, image, c->d_tm.as<float>(), sdf_res, sdf_params, iso, band, level_counts, n_levels);
+    if (!rc) rc = mc_run(c, c->ad_grid.as<float>(), (int)R, sdf_params, iso, nullptr, nullptr);
+  } else if (!rc) {
+    rc = adaptive_mesh_run(c, nullptr, image, c->d_tm.as<float>(), sdf_res, sdf_params, iso, band, level_counts, n_levels,
+                           nullptr, nullptr);
+  }
+  if (!rc && cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    set_error("mesh_grid_adaptive: stream synchronisation failed");
+    rc = -1;
+  }
+  if (!rc) rc = check_status(c);    // the f16f8 overflow status: the mesh was built from invalid values
+  return finish_mesh_call(c, rc, n_verts, n_faces);
 }
 
 // ---- cross-process device buffers (multi-GPU gather without a collective) -------------------------------------------

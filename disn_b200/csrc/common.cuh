@@ -279,6 +279,17 @@ struct disn_ctx {
   cudaEvent_t ad_ev[7] = {};
   int32_t ad_R = 0, ad_levels = 0;
   disn::DevBuffer d_mc_in;
+  // coarse-to-fine mesh without a dense grid (adaptive_mesh.cu): block states of every level, the coarse lattice values,
+  // each level's active blocks and value table, the sort buffers of the level lists and then of the crossing cells, the
+  // crossing edges, the network's coordinate and value chunks, cases and face offsets of the cells, scan scratch, device
+  // counters with their pinned mirror and the phase events.  am_nv: vertices of the last call (-1: none or failed),
+  // am_edges_sorted: its sorted crossing edges (vertex v = edge of rank v)
+  disn::DevBuffer am_state, am_coarse, am_active[4], am_table[4], am_keys[2], am_edges[2], am_sort_tmp, am_xyz, am_vals,
+      am_case, am_tri, am_sums, am_cnt;
+  disn::PinnedBuffer am_host;
+  cudaEvent_t am_ev[4] = {};
+  int64_t am_nv = -1;
+  const unsigned long long* am_edges_sorted = nullptr;
   // nn_distance / cam scratch (persistent, grows)
   disn::DevBuffer nn_scratch;
   disn::DevBuffer dec_scratch;  // explicit-feature decoder staging (decoder.cu)
@@ -345,4 +356,13 @@ int eval_indexed(disn_ctx* c, int image, int R, const float* d_tm, const int32_t
 // the network (eval_indexed, with d_tm and the axis tables as above).  The filled grid stays in c->ad_grid.
 int adaptive_run(disn_ctx* c, const float* field, int image, const float* d_tm, int32_t res, const double* sdf_params,
                  float iso, double band, int64_t* level_counts, int32_t* n_levels);
+// adaptive_mesh.cu: the mesh of adaptive_run's grid followed by mc_run, built from the surface blocks alone (s0 >= 2);
+// field / image / d_tm as for adaptive_run.  The mesh becomes the resident mesh (c->mc_verts / c->mc_faces).
+int adaptive_mesh_run(disn_ctx* c, const float* field, int image, const float* d_tm, int32_t res, const double* sdf_params,
+                      float iso, double band, int64_t* level_counts, int32_t* n_levels, int64_t* n_verts,
+                      int64_t* n_faces);
+// api.cu: the end of a call that builds the resident mesh from rc: empties the mesh on failure, reports its counts
+int finish_mesh_call(disn_ctx* c, int rc, int64_t* n_verts, int64_t* n_faces);
+// bytes held by the buffers of adaptive_mesh_run
+size_t adaptive_mesh_bytes(const disn_ctx* c);
 }  // namespace disn

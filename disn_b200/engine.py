@@ -522,6 +522,33 @@ class Engine:
                                                counts.ctypes.data_as(C.c_void_p), C.byref(nl)))
         return int(out.value), [int(v) for v in counts[:nl.value]]
 
+    def mesh_grid_adaptive(self, sdf_params, trans_mat, sdf_res: int, iso: float = 0.0, band: float = 1.0, image: int = 0,
+                           fetch: bool = True):
+        """Coarse-to-fine mesh of encoded image `image` without a dense grid (DESIGN.md §4.10): bit for bit the mesh
+        marching_cubes makes of eval_grid_adaptive's grid, with memory proportional to the evaluated points; sdf_res up to
+        2048.  The mesh stays resident (clean_mesh, write_mesh_obj) -> (verts, faces, level_counts), or with fetch=False
+        ((n_verts, n_faces), level_counts)."""
+        sp = np.ascontiguousarray(sdf_params, dtype=np.float64).reshape(6)
+        t = _f32(trans_mat).reshape(4, 3)
+        counts = np.zeros(5, np.int64)
+        nl = C.c_int32(0)
+        # the library reports the resident counts whenever it may have changed the mesh, also when the call fails (the
+        # mesh is then empty); an argument error leaves both, so start from the counts of the mesh held now
+        nv, nf = C.c_int64(self._mesh_verts), C.c_int64(self._mesh_faces)
+        rc = self.lib.disn_mesh_grid_adaptive(self._h, sp.ctypes.data_as(C.POINTER(C.c_double)), t.ctypes.data_as(C.c_void_p),
+                                              image, sdf_res, float(iso), float(band), counts.ctypes.data_as(C.c_void_p),
+                                              C.byref(nl), C.byref(nv), C.byref(nf))
+        self._mesh_verts, self._mesh_faces = nv.value, nf.value
+        check(rc)
+        levels = [int(v) for v in counts[:nl.value]]
+        if not fetch:
+            return (nv.value, nf.value), levels
+        verts = np.empty((nv.value, 3), dtype=np.float32)
+        faces = np.empty((nf.value, 3), dtype=np.int32)
+        if nv.value and nf.value:
+            check(self.lib.disn_mc_fetch(self._h, verts.ctypes.data_as(C.c_void_p), faces.ctypes.data_as(C.c_void_p)))
+        return verts, faces, levels
+
     def fetch(self, dev_ptr: int, shape, dtype=np.float32) -> np.ndarray:
         out = np.empty(shape, dtype=dtype)
         check(self.lib.disn_fetch(self._h, C.c_void_p(dev_ptr), out.ctypes.data_as(C.c_void_p), out.nbytes))

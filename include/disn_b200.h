@@ -152,6 +152,19 @@ int disn_eval_grid_indexed(disn_ctx* ctx, const double* sdf_params, const float*
 int disn_eval_grid_adaptive(disn_ctx* ctx, const double* sdf_params, const float* trans_mat, int32_t image,
                             int32_t sdf_res, float iso, double band, float** grid_dev, int64_t* level_counts,
                             int32_t* n_levels);
+/* Coarse-to-fine mesh of encoded image `image` without a dense grid (DESIGN.md 4.10): the levels of
+ * disn_eval_grid_adaptive, with the evaluated values kept in tables proportional to their number, then marching cubes on
+ * the cells that can cross iso only.  The welded mesh becomes the resident mesh (disn_mc_fetch, disn_mc_write_obj,
+ * disn_mesh_clean) and equals, bit for bit, the mesh disn_mc_run makes of disn_eval_grid_adaptive's grid: vertices, faces,
+ * their order and level_counts (at least 5 entries; *n_levels their number), in every precision and for every band.
+ * 1 <= sdf_res <= 2048, iso finite, band >= 0.  An odd sdf_res (s0 = 1) evaluates the dense grid as
+ * disn_eval_grid_adaptive does and needs sdf_res <= 1125.  Refuses meshes with 2^31 or more vertices or faces.  Once the
+ * arguments are accepted, *n_verts / *n_faces (each may be NULL) receive the resident mesh's counts, also on failure: a
+ * failed call (out of memory, a refused size, the DISN_PREC_F16F8 overflow status) leaves the resident mesh empty.
+ * Synchronises once per level and twice for the mesh. */
+int disn_mesh_grid_adaptive(disn_ctx* ctx, const double* sdf_params, const float* trans_mat, int32_t image,
+                            int32_t sdf_res, float iso, double band, int64_t* level_counts, int32_t* n_levels,
+                            int64_t* n_verts, int64_t* n_faces);
 int disn_mc_run(disn_ctx* ctx, const float* sdf, int32_t R, const double* bbox, float iso, uint32_t flags,
                 int64_t* n_verts, int64_t* n_faces);
 int disn_mc_fetch(disn_ctx* ctx, float* verts, int32_t* faces);

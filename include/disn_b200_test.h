@@ -37,6 +37,20 @@ int disn_adaptive_from_field(disn_ctx* ctx, const float* field, int32_t sdf_res,
                              double band, uint32_t flags, float** grid_dev, int64_t* level_counts, int32_t* n_levels);
 int disn_adaptive_phase_ms(disn_ctx* ctx, float* ms, int32_t* n);
 
+/* Diagnostics of the coarse-to-fine mesh (disn_mesh_grid_adaptive):
+ *   disn_mesh_adaptive_from_field: the same mesh with values read from field [R,R,R] (host, or device with
+ *     DISN_DEVICE_PTR) instead of the network, (sdf_res+1)^3 < 2^31, sdf_res even;
+ *   disn_mesh_adaptive_phase_ms: device-event milliseconds of the last call's phases -- levels, candidate cells, mesh --
+ *     into ms[3];
+ *   disn_mesh_adaptive_bytes: bytes held by the call's buffers (the resident mesh not included);
+ *   disn_mesh_adaptive_edges: the edge ids ((z*R + y)*R + x)*3 + axis of vertices [first, first + n) of the last call. */
+int disn_mesh_adaptive_from_field(disn_ctx* ctx, const float* field, int32_t sdf_res, const double* sdf_params, float iso,
+                                  double band, uint32_t flags, int64_t* level_counts, int32_t* n_levels, int64_t* n_verts,
+                                  int64_t* n_faces);
+int disn_mesh_adaptive_phase_ms(disn_ctx* ctx, float* ms);
+int disn_mesh_adaptive_bytes(disn_ctx* ctx, int64_t* bytes);
+int disn_mesh_adaptive_edges(disn_ctx* ctx, int64_t first, int64_t n, int64_t* out);
+
 #ifdef __cplusplus
 }
 #endif
