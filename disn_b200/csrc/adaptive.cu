@@ -158,7 +158,7 @@ int evaluate_list(disn_ctx* c, const float* field, int image, const float* d_tm,
   const float* vals = nullptr;
   if (!field) {
     if (c->ad_vals.ensure((size_t)n * sizeof(float))) return -1;
-    if (eval_indexed(c, image, R, d_tm, list, n, c->ad_vals.as<float>())) return -1;
+    if (eval_grid_points(c, image, R, d_tm, list, n, c->ad_vals.as<float>())) return -1;
     vals = c->ad_vals.as<float>();
   }
   scatter_kernel<<<blocks_of(n), AD_THREADS, 0, c->stream>>>(list, n, vals, field, grid);
@@ -203,7 +203,7 @@ int adaptive_run(disn_ctx* c, const float* field, int image, const float* d_tm, 
 
   if (s0 == 1) {            // no power of two divides res: the dense grid
     if (field) DISN_CUDA_OK(cudaMemcpyAsync(grid, field, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    else if (eval_indexed(c, image, R, d_tm, nullptr, n, grid)) return -1;
+    else if (eval_grid_points<int32_t>(c, image, R, d_tm, nullptr, n, grid)) return -1;
     DISN_CUDA_OK(cudaMemsetAsync(mark, 1, (size_t)n, st));
     DISN_CUDA_OK(cudaEventRecord(c->ad_ev[1], st));
     level_counts[0] = n;

@@ -10,8 +10,8 @@
 //     means the point was never evaluated and takes the fill rule;
 //   * marching cubes visits only the candidate cells K (§4.10) and numbers vertices by the rank of their edge id among
 //     the sorted crossing edges, faces by cell then table order: mc.cu's mesh of the dense adaptive grid, bit for bit.
-// The network evaluates each list in chunks of explicit points built from the float32 axis tables (point_of then reads
-// the floats grid mode reads), one host synchronisation per level and two for the mesh.
+// The network evaluates the lattice and each sorted list through eval_grid_points (api.cu), one host synchronisation per
+// level and two for the mesh.
 #include <algorithm>
 #include <cmath>
 
@@ -25,7 +25,7 @@ namespace disn {
 namespace {
 
 constexpr int AM_THREADS = 256;
-constexpr int64_t AM_CHUNK = (int64_t)1 << 24;     // points per network call (12 B of coordinates each)
+constexpr int64_t AM_CHUNK = (int64_t)1 << 24;     // points per network call (4 B of values each)
 constexpr unsigned long long AM_EMPTY = ~0ull;     // free hash slot
 
 inline unsigned blocks_of(int64_t n) { return (unsigned)((n + AM_THREADS - 1) / AM_THREADS); }
@@ -151,23 +151,6 @@ __device__ __forceinline__ bool block_is_active(const uint8_t* st, int nb, int b
 }
 
 // ---- coarse lattice and level lists ---------------------------------------------------------------------------------
-
-// xyz rows of points [j0, j0 + n): keys[j] (linear indices), or the stride-s0 lattice point j in lattice order
-__global__ void __launch_bounds__(AM_THREADS) xyz_kernel(const unsigned long long* __restrict__ keys, int64_t j0, int64_t n,
-                                                         int R, int s0, int M, const float* __restrict__ axes,
-                                                         float* __restrict__ xyz) {
-  const int64_t j = (int64_t)blockIdx.x * AM_THREADS + threadIdx.x;
-  if (j >= n) return;
-  int x, y, z;
-  if (keys) {
-    const unsigned long long i = keys[j0 + j];
-    x = (int)(i % R); y = (int)((i / R) % R); z = (int)(i / ((unsigned long long)R * R));
-  } else {
-    const int64_t i = j0 + j;
-    x = (int)(i % M) * s0; y = (int)((i / M) % M) * s0; z = (int)(i / ((int64_t)M * M)) * s0;
-  }
-  xyz[j * 3 + 0] = axes[x]; xyz[j * 3 + 1] = axes[R + y]; xyz[j * 3 + 2] = axes[2 * R + z];
-}
 
 // the lattice values read from a given dense field
 __global__ void __launch_bounds__(AM_THREADS) lattice_from_field_kernel(const float* __restrict__ field, int R, int s0, int M,
@@ -458,46 +441,27 @@ int sort_keys(disn_ctx* c, DevBuffer (&keys)[2], int64_t n, int bits, unsigned l
   return 0;
 }
 
-// the network at n explicit points xyz of one image -> out (pred / sdf_weight), as eval_indexed does in grid mode
-int evaluate_points(disn_ctx* c, int image, const float* d_tm, const float* xyz, int64_t n, float* out) {
-  PointJob job{};
-  job.B = 1; job.N = n; job.pts = xyz; job.pts_rot = nullptr;
-  job.gbias = c->gbias.as<float>() + (int64_t)image * kHidden;
-  job.pmap = c->pmap.as<float>() + (int64_t)image * c->cfg.img_h * c->cfg.img_w * kHidden;
-  job.trans_mat = d_tm;
-  job.out_pred = out;
-  job.out_div = c->cfg.sdf_weight;
-  return run_point_job(c, job);
-}
-
-// values of n points (keys, or the coarse lattice with keys == nullptr) in chunks: xyz rows, then the network into
-// out[j] (lattice) or the chunk buffer and from there into the level's table
-int evaluate_chunks(disn_ctx* c, int image, const float* d_tm, const Field& f, const unsigned long long* keys, int64_t n,
-                    float* out, unsigned long long* tkeys, float* tvals, unsigned long long cap) {
+// the network at a level's n sorted keys, one chunk at a time through am_vals into the level's table
+int evaluate_level(disn_ctx* c, int image, const float* d_tm, int R, const unsigned long long* keys, int64_t n,
+                   unsigned long long* tkeys, float* tvals, unsigned long long cap) {
   const int64_t chunk = std::min<int64_t>(n, AM_CHUNK);
-  if (c->am_xyz.ensure((size_t)chunk * 3 * sizeof(float)) || (keys && c->am_vals.ensure((size_t)chunk * sizeof(float))))
-    return -1;
+  if (c->am_vals.ensure((size_t)chunk * sizeof(float))) return -1;
   for (int64_t j0 = 0; j0 < n; j0 += chunk) {
     const int64_t m = std::min<int64_t>(chunk, n - j0);
-    xyz_kernel<<<blocks_of(m), AM_THREADS, 0, c->stream>>>(keys, j0, m, f.R, f.s0, f.M, c->d_axes.as<float>(),
-                                                           c->am_xyz.as<float>());
+    if (eval_grid_points(c, image, R, d_tm, keys + j0, m, c->am_vals.as<float>())) return -1;
+    table_insert_kernel<<<blocks_of(m), AM_THREADS, 0, c->stream>>>(keys + j0, m, c->am_vals.as<float>(), nullptr, tkeys,
+                                                                    tvals, cap);
     c->launches++;
     DISN_CUDA_OK(cudaGetLastError());
-    float* dst = keys ? c->am_vals.as<float>() : out + j0;
-    if (evaluate_points(c, image, d_tm, c->am_xyz.as<float>(), m, dst)) return -1;
-    if (keys) {
-      table_insert_kernel<<<blocks_of(m), AM_THREADS, 0, c->stream>>>(keys + j0, m, dst, nullptr, tkeys, tvals, cap);
-      c->launches++;
-      DISN_CUDA_OK(cudaGetLastError());
-    }
   }
   return 0;
 }
 
 }  // namespace
 
+// the network's coordinate rows (c->d_rows) are held for this call's evaluations, so they count here
 size_t adaptive_mesh_bytes(const disn_ctx* c) {
-  size_t b = c->am_state.bytes() + c->am_coarse.bytes() + c->am_xyz.bytes() + c->am_vals.bytes() + c->am_sort_tmp.bytes() +
+  size_t b = c->am_state.bytes() + c->am_coarse.bytes() + c->d_rows.bytes() + c->am_vals.bytes() + c->am_sort_tmp.bytes() +
              c->am_case.bytes() + c->am_tri.bytes() + c->am_sums.bytes() + c->am_cnt.bytes();
   for (int k = 0; k < 2; ++k) b += c->am_keys[k].bytes() + c->am_edges[k].bytes();
   for (int l = 0; l < AD_MAX_LEVELS; ++l) b += c->am_table[l].bytes() + c->am_active[l].bytes();
@@ -542,7 +506,7 @@ int adaptive_mesh_run(disn_ctx* c, const float* field, int image, const float* d
     lattice_from_field_kernel<<<blocks_of(nM), AM_THREADS, 0, st>>>(field, R, f.s0, f.M, coarse);
     c->launches++;
     DISN_CUDA_OK(cudaGetLastError());
-  } else if (evaluate_chunks(c, image, d_tm, f, nullptr, nM, coarse, nullptr, nullptr, 0)) {
+  } else if (eval_grid_points<unsigned long long>(c, image, R, d_tm, nullptr, nM, coarse, f.s0)) {
     return -1;
   }
   level_counts[0] = nM;
@@ -590,7 +554,7 @@ int adaptive_mesh_run(disn_ctx* c, const float* field, int image, const float* d
       table_insert_kernel<<<blocks_of(n_new), AM_THREADS, 0, st>>>(keys, n_new, nullptr, field, tkeys, tvals, cap);
       c->launches++;
       DISN_CUDA_OK(cudaGetLastError());
-    } else if (evaluate_chunks(c, image, d_tm, f, keys, n_new, nullptr, tkeys, tvals, cap)) {
+    } else if (evaluate_level(c, image, d_tm, R, keys, n_new, tkeys, tvals, cap)) {
       return -1;
     }
     f.t[l] = Table{tkeys, tvals, cap};

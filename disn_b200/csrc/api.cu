@@ -1,4 +1,5 @@
 // C ABI of the DISN hot-path library (see include/disn_b200.h for the reference call sites).
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -258,13 +259,7 @@ int disn::run_point_job(disn_ctx* c, PointJob& job) {
   fill_stream(c, "sdfprediction", job.g);
   fill_stream(c, "sdfprediction_imgfeat", job.l);
   job.status = c->d_status.as<int>();
-  if (c->cfg.precision == DISN_PREC_FP32) {
-    if (launch_point_fp32(c, job)) return -1;
-    if (job.idx)      // only an indexed job can raise a status on the fp32 path
-      DISN_CUDA_OK(cudaMemcpyAsync(c->h_status.as<int>(), job.status, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    return 0;
-  }
-  if (launch_point_tc(c, job)) return -1;
+  if (c->cfg.precision == DISN_PREC_FP32 ? launch_point_fp32(c, job) : launch_point_tc(c, job)) return -1;
   // the status word travels to the pinned mirror behind the kernel; whoever synchronises next checks it
   DISN_CUDA_OK(cudaMemcpyAsync(c->h_status.as<int>(), job.status, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   return 0;
@@ -616,7 +611,7 @@ int disn_eval_grid_indexed(disn_ctx* c, const double* sdf_params, const float* t
   if (n == 0) return 0;
   const int R = sdf_res + 1;
   if (grid_axes(c, sdf_params, 1, R)) return -1;
-  if (flags & DISN_DEVICE_PTR) return eval_indexed(c, image, R, trans_mat, idx, n, out);
+  if (flags & DISN_DEVICE_PTR) return eval_grid_points(c, image, R, trans_mat, idx, n, out);
   const int64_t R3 = (int64_t)R * R * R;
   for (int64_t i = 0; i < n; ++i)
     DISN_REQUIRE(idx[i] >= 0 && idx[i] < R3, "eval_grid_indexed: index " + std::to_string(idx[i]) + " at position " +
@@ -624,7 +619,7 @@ int disn_eval_grid_indexed(disn_ctx* c, const double* sdf_params, const float* t
   if (c->d_idx.ensure((size_t)n * sizeof(int32_t)) || ensure_point_scratch(c, n)) return -1;
   DISN_CUDA_OK(cudaMemcpyAsync(c->d_idx.as<int32_t>(), idx, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaMemcpyAsync(c->d_tm.as<float>(), trans_mat, 12 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  if (eval_indexed(c, image, R, c->d_tm.as<float>(), c->d_idx.as<int32_t>(), n, c->d_out.as<float>())) return -1;
+  if (eval_grid_points(c, image, R, c->d_tm.as<float>(), c->d_idx.as<int32_t>(), n, c->d_out.as<float>())) return -1;
   DISN_CUDA_OK(cudaMemcpyAsync(out, c->d_out.as<float>(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
   return check_status(c);
@@ -772,15 +767,71 @@ int disn::grid_axes(disn_ctx* c, const double* sdf_params, int B, int R) {
   return 0;
 }
 
-// One image of the encoded batch as a batch of one: its gbias / pmap rows, its matrix and the first axis tables.
-int disn::eval_indexed(disn_ctx* c, int image, int R, const float* d_tm, const int32_t* idx, int64_t n, float* out) {
+namespace disn {
+namespace {
+
+constexpr int ROW_THREADS = 256;
+constexpr int64_t ROW_CHUNK = (int64_t)1 << 24;   // grid points per network call (12 B of coordinates each)
+
+// x,y,z rows of points [j0, j0 + n) from the axis tables: grid point idx[j] (an index outside the grid raises the status
+// and reads point 0), or point j of the stride-s lattice.  The floats are the ones grid mode reads, so explicit-point
+// evaluation of the rows gives grid mode's values.
+template <class Index>
+__global__ void __launch_bounds__(ROW_THREADS) grid_rows_kernel(const Index* __restrict__ idx, int64_t j0, int64_t n, int R,
+                                                                int s, const float* __restrict__ axes,
+                                                                float* __restrict__ xyz, int* __restrict__ status) {
+  const int64_t j = (int64_t)blockIdx.x * ROW_THREADS + threadIdx.x;
+  if (j >= n) return;
+  int x, y, z;
+  if (idx) {
+    int64_t i = (int64_t)idx[j0 + j];
+    if ((uint64_t)i >= (uint64_t)R * R * R) {
+      atomicOr(status, DISN_STATUS_BAD_INDEX);
+      i = 0;
+    }
+    x = (int)(i % R); y = (int)((i / R) % R); z = (int)(i / ((int64_t)R * R));
+  } else {
+    const int M = (R - 1) / s + 1;
+    const int64_t i = j0 + j;
+    x = (int)(i % M) * s; y = (int)((i / M) % M) * s; z = (int)(i / ((int64_t)M * M)) * s;
+  }
+  xyz[j * 3 + 0] = axes[x]; xyz[j * 3 + 1] = axes[R + y]; xyz[j * 3 + 2] = axes[2 * R + z];
+}
+
+}  // namespace
+
+// One image of the encoded batch as a batch of one: its gbias / pmap rows, its matrix and the first axis tables.  The
+// dense grid runs in grid mode; listed and lattice points go through explicit-point rows, one chunk at a time.
+template <class Index>
+int eval_grid_points(disn_ctx* c, int image, int R, const float* d_tm, const Index* idx, int64_t n, float* out, int s) {
   if (n == 0) return 0;
   PointJob job{};
-  job.B = 1; job.N = n; job.R = R; job.z0 = 0; job.idx = idx; job.axes = c->d_axes.as<float>();
+  job.B = 1;
   job.gbias = c->gbias.as<float>() + (int64_t)image * kHidden;
   job.pmap = c->pmap.as<float>() + (int64_t)image * c->cfg.img_h * c->cfg.img_w * kHidden;
   job.trans_mat = d_tm;
-  job.out_pred = out;
   job.out_div = c->cfg.sdf_weight;
-  return run_point_job(c, job);
+  if (!idx && s == 1) {
+    job.N = n; job.R = R; job.z0 = 0; job.axes = c->d_axes.as<float>();
+    job.out_pred = out;
+    return run_point_job(c, job);
+  }
+  const int64_t chunk = std::min<int64_t>(n, ROW_CHUNK);
+  if (c->d_rows.ensure((size_t)chunk * 3 * sizeof(float))) return -1;
+  for (int64_t j0 = 0; j0 < n; j0 += chunk) {
+    const int64_t m = std::min<int64_t>(chunk, n - j0);
+    grid_rows_kernel<Index><<<(unsigned)((m + ROW_THREADS - 1) / ROW_THREADS), ROW_THREADS, 0, c->stream>>>(
+        idx, j0, m, R, s, c->d_axes.as<float>(), c->d_rows.as<float>(), c->d_status.as<int>());
+    c->launches++;
+    DISN_CUDA_OK(cudaGetLastError());
+    job.N = m; job.pts = c->d_rows.as<float>(); job.pts_rot = nullptr;
+    job.out_pred = out + j0;
+    if (run_point_job(c, job)) return -1;
+  }
+  return 0;
 }
+template int eval_grid_points<int32_t>(disn_ctx*, int, int, const float*, const int32_t*, int64_t, float*, int);
+template int eval_grid_points<unsigned long long>(disn_ctx*, int, int, const float*, const unsigned long long*, int64_t,
+                                                  float*, int);
+
+}  // namespace disn

@@ -155,9 +155,7 @@ struct PointJob {
   const float* trans_mat; // [B,4,3] device
   const float* axes;      // grid mode: [B,3,R] float32 linspace tables (x,y,z)
   int32_t R;              // grid mode: points per axis
-  int32_t z0;             // grid mode: first z plane
-  const int32_t* idx;     // grid mode: point n is grid point idx[n] = (z*R + y)*R + x (z0 = 0), or nullptr: point n is
-                          // z0*R^2 + n (the dense slab)
+  int32_t z0;             // grid mode: first z plane; point n is grid point z0*R^2 + n (the dense slab)
   int64_t N;              // points per image in this call
   int32_t B;
   // per-image encoder products
@@ -181,17 +179,40 @@ struct PointJob {
 };
 
 constexpr int DISN_STATUS_FP16_OVERFLOW = 1;   // DISN_PREC_F16F8: an activation exceeded fp16's range
-constexpr int DISN_STATUS_BAD_INDEX = 2;       // grid mode with idx: an index outside [0, R^3) (evaluated as point 0)
+constexpr int DISN_STATUS_BAD_INDEX = 2;       // eval_grid_points: a listed index outside [0, R^3) (evaluated as point 0)
 
-// linear grid index of point n of a grid-mode job (see PointJob::idx)
-__device__ __forceinline__ int64_t grid_index(const PointJob& job, int64_t n) {
-  if (!job.idx) return n;
-  const int64_t i = job.idx[n];
-  if (i < 0 || i >= (int64_t)job.R * job.R * job.R) {
-    if (job.status) atomicOr(job.status, DISN_STATUS_BAD_INDEX);
-    return 0;
+// query point n of image b of a point job: (x, y, z) is projected, (xr, yr, zr) feeds the MLP; zeros past the end
+__device__ __forceinline__ void point_of(const PointJob& job, int b, int64_t n, float& x, float& y, float& z, float& xr,
+                                         float& yr, float& zr) {
+  x = y = z = xr = yr = zr = 0.f;
+  if (n >= job.N) return;
+  if (job.pts) {
+    const float* q = job.pts + ((int64_t)b * job.N + n) * 3;
+    x = q[0]; y = q[1]; z = q[2];
+    if (job.pts_rot) {
+      const float* r = job.pts_rot + ((int64_t)b * job.N + n) * 3;
+      xr = r[0]; yr = r[1]; zr = r[2];
+    } else { xr = x; yr = y; zr = z; }
+  } else {
+    const int R = job.R;
+    const int ix = (int)(n % R);
+    const int64_t tt = n / R;
+    const int iy = (int)(tt % R);
+    const int iz = (int)(tt / R) + job.z0;
+    const float* ax = job.axes + (int64_t)b * 3 * R;
+    x = ax[ix]; y = ax[R + iy]; z = ax[2 * R + iz];
+    xr = x; yr = y; zr = z;
   }
-  return i;
+}
+
+// image coordinates of a point (models/model_normalization.py:241-251): [x,y,z,1] . T (T: [4,3], fp32 multiply-adds in
+// k order like a plain matmul), divided by the depth and clamped to [0, clamp_max]
+__device__ __forceinline__ void project(const float* T, float clamp_max, float x, float y, float z, float& u, float& v) {
+  const float q0 = fmaf(z, T[6], fmaf(y, T[3], x * T[0])) + T[9];
+  const float q1 = fmaf(z, T[7], fmaf(y, T[4], x * T[1])) + T[10];
+  const float q2 = fmaf(z, T[8], fmaf(y, T[5], x * T[2])) + T[11];
+  u = fminf(clamp_max, fmaxf(0.f, q0 / q2));
+  v = fminf(clamp_max, fmaxf(0.f, q1 / q2));
 }
 
 }  // namespace disn
@@ -271,6 +292,7 @@ struct disn_ctx {
   // device-resident SDF grid of disn_eval_grid_resident and host staging for the marching-cubes input
   disn::DevBuffer d_grid;
   disn::DevBuffer d_idx;        // host-index staging of disn_eval_grid_indexed
+  disn::DevBuffer d_rows;       // eval_grid_points: x,y,z rows of one chunk of listed grid points
   // coarse-to-fine grid (adaptive.cu): the filled grid, one byte per point (1 = evaluated), the block states of every
   // level, the per-level index list and its values, compaction counts and scan scratch, host-field staging, the
   // pinned level total and the phase events; ad_R / ad_levels describe the last call
@@ -281,11 +303,11 @@ struct disn_ctx {
   disn::DevBuffer d_mc_in;
   // coarse-to-fine mesh without a dense grid (adaptive_mesh.cu): block states of every level, the coarse lattice values,
   // each level's active blocks and value table, the sort buffers of the level lists and then of the crossing cells, the
-  // crossing edges, the network's coordinate and value chunks, cases and face offsets of the cells, scan scratch, device
-  // counters with their pinned mirror and the phase events.  am_nv: vertices of the last call (-1: none or failed),
-  // am_edges_sorted: its sorted crossing edges (vertex v = edge of rank v)
-  disn::DevBuffer am_state, am_coarse, am_active[4], am_table[4], am_keys[2], am_edges[2], am_sort_tmp, am_xyz, am_vals,
-      am_case, am_tri, am_sums, am_cnt;
+  // crossing edges, the network's value chunk, cases and face offsets of the cells, scan scratch, device counters with
+  // their pinned mirror and the phase events.  am_nv: vertices of the last call (-1: none or failed), am_edges_sorted:
+  // its sorted crossing edges (vertex v = edge of rank v)
+  disn::DevBuffer am_state, am_coarse, am_active[4], am_table[4], am_keys[2], am_edges[2], am_sort_tmp, am_vals, am_case,
+      am_tri, am_sums, am_cnt;
   disn::PinnedBuffer am_host;
   cudaEvent_t am_ev[4] = {};
   int64_t am_nv = -1;
@@ -349,11 +371,15 @@ int sdf_strided(disn_ctx* c, const float* sdf, int32_t R, int32_t reduce, bool d
 void axis_table(double start, double stop, int num, float* out);
 // api.cu: the float32 axis tables of B boxes in c->d_axes (uploaded only when boxes or R change)
 int grid_axes(disn_ctx* c, const double* sdf_params, int B, int R);
-// api.cu: grid points idx[0..n) (device) of encoded image `image` -> out[0..n) (device) = pred/sdf_weight; the axis tables
-// of that image's box must be in c->d_axes (grid_axes with B = 1); d_tm: the image's [4,3] matrix on the device
-int eval_indexed(disn_ctx* c, int image, int R, const float* d_tm, const int32_t* idx, int64_t n, float* out);
+// api.cu: n grid points of encoded image `image` -> out[0..n) (device) = pred/sdf_weight, bitwise disn_eval_grid's values.
+// Point j is grid point idx[j] = (z*R + y)*R + x (device; Index = int32_t or unsigned long long), or with idx == nullptr
+// point j of the stride-s lattice in (z, y, x) order (s = 1: the dense grid).  The axis tables of the image's box must be
+// in c->d_axes (grid_axes with B = 1); d_tm: the image's [4,3] matrix on the device.  A listed index outside [0, R^3)
+// raises DISN_STATUS_BAD_INDEX and is evaluated as point 0.
+template <class Index>
+int eval_grid_points(disn_ctx* c, int image, int R, const float* d_tm, const Index* idx, int64_t n, float* out, int s = 1);
 // adaptive.cu: coarse-to-fine grid of one image; values come from `field` (device [R,R,R]) when it is non-null, else from
-// the network (eval_indexed, with d_tm and the axis tables as above).  The filled grid stays in c->ad_grid.
+// the network (eval_grid_points, with d_tm and the axis tables as above).  The filled grid stays in c->ad_grid.
 int adaptive_run(disn_ctx* c, const float* field, int image, const float* d_tm, int32_t res, const double* sdf_params,
                  float iso, double band, int64_t* level_counts, int32_t* n_levels);
 // adaptive_mesh.cu: the mesh of adaptive_run's grid followed by mc_run, built from the surface blocks alone (s0 >= 2);

@@ -68,15 +68,8 @@ __global__ void point_img_feat_kernel(TapLevels lv, const float* __restrict__ uv
 __global__ void img_points_kernel(const float* __restrict__ pts, const float* __restrict__ tm, float* __restrict__ uv, int B,
                                   int64_t N, float clamp_max) {
   const int64_t total = (int64_t)B * N;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const float* T = tm + (i / N) * 12;
-    const float x = pts[i * 3], y = pts[i * 3 + 1], z = pts[i * 3 + 2];
-    const float q0 = fmaf(z, T[6], fmaf(y, T[3], x * T[0])) + T[9];
-    const float q1 = fmaf(z, T[7], fmaf(y, T[4], x * T[1])) + T[10];
-    const float q2 = fmaf(z, T[8], fmaf(y, T[5], x * T[2])) + T[11];
-    uv[i * 2] = fminf(clamp_max, fmaxf(0.f, q0 / q2));
-    uv[i * 2 + 1] = fminf(clamp_max, fmaxf(0.f, q1 / q2));
-  }
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
+    project(tm + (i / N) * 12, clamp_max, pts[i * 3], pts[i * 3 + 1], pts[i * 3 + 2], uv[i * 2], uv[i * 2 + 1]);
 }
 
 }  // namespace

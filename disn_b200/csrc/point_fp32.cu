@@ -212,34 +212,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) point_fp32_kernel(PointJob job, i
     if (threadIdx.x < TP) {
       const int p = threadIdx.x;
       const int64_t n = n0 + p;
-      float x = 0.f, y = 0.f, z = 0.f, xr = 0.f, yr = 0.f, zr = 0.f;
-      if (n < job.N) {
-        if (job.pts) {
-          const float* q = job.pts + ((int64_t)b * job.N + n) * 3;
-          x = q[0]; y = q[1]; z = q[2];
-          if (job.pts_rot) {
-            const float* r = job.pts_rot + ((int64_t)b * job.N + n) * 3;
-            xr = r[0]; yr = r[1]; zr = r[2];
-          } else { xr = x; yr = y; zr = z; }
-        } else {
-          const int R = job.R;
-          const int64_t m = grid_index(job, n);
-          int ix = (int)(m % R);
-          int64_t t = m / R;
-          int iy = (int)(t % R);
-          int iz = (int)(t / R) + job.z0;
-          const float* ax = job.axes + (int64_t)b * 3 * R;
-          x = ax[ix]; y = ax[R + iy]; z = ax[2 * R + iz];
-          xr = x; yr = y; zr = z;
-        }
-      }
-      const float* T = job.trans_mat + b * 12;
-      // [x,y,z,1] . T(4x3); fp32 multiply-adds in k order like a plain matmul
-      float q0 = fmaf(z, T[6], fmaf(y, T[3], x * T[0])) + T[9];
-      float q1 = fmaf(z, T[7], fmaf(y, T[4], x * T[1])) + T[10];
-      float q2 = fmaf(z, T[8], fmaf(y, T[5], x * T[2])) + T[11];
-      float u = fminf(job.clamp_max, fmaxf(0.f, q0 / q2));
-      float v = fminf(job.clamp_max, fmaxf(0.f, q1 / q2));
+      float x, y, z, xr, yr, zr, u, v;
+      point_of(job, b, n, x, y, z, xr, yr, zr);
+      project(job.trans_mat + b * 12, job.clamp_max, x, y, z, u, v);
       s.px[p] = xr; s.py[p] = yr; s.pz[p] = zr;
       s.u[p] = u; s.v[p] = v;
       if (job.out_uv && n < job.N) {

@@ -28,7 +28,6 @@
 //     (constant bank, warp-uniform indexed loads).
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -53,8 +52,10 @@ constexpr int X8_TILE = 4096;         // 64 rows x 64 k x 1 B (SW64)
 constexpr int X_SLICE = 2 * X_TILE;   // one 64-wide K slice: [hi | lo] or [fp16 | e5m2 residual | e5m2 copy]
 constexpr int STAGES_PER_STREAM = 33; // 1 + 8 + 16 + 8 (K slice, 256-wide N block) stages
 constexpr int HS_PER_TILE = 2 * 2 * STAGES_PER_STREAM;
-constexpr int CORR_DEFAULT = 0xDF;    // correction mask of DISN_PREC_F16F8 (see kCorr below): every correction except the
-                                      // a.(w - h(w)) product of fold2/conv1
+// correction products DISN_PREC_F16F8 keeps in each tensor layer l = 0..3 (fold1/conv2, fold1/conv3, fold2/conv1,
+// fold2/conv2): bit 2l (a - h(a)).w ("first"), bit 2l+1 a.(w - h(w)) ("second").  Every correction except the second
+// product of fold2/conv1 (DESIGN.md section 3).
+constexpr int CORR_DEFAULT = 0xDF;
 // shared-memory table of small fp32 parameters per stream
 constexpr int SB_B2 = 0, SB_B3 = 256, SB_B4 = 768, SB_B5 = 1280, SB_W6 = 1536, SB_W1 = 1792, SB_B1 = 1984, SB_STRIDE = 2048;
 __host__ __device__ constexpr int layer_k(int l) { return l == 0 ? 64 : (l == 1 ? 256 : 512); }
@@ -77,42 +78,7 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// query point n of image b: (x, y, z) is projected, (xr, yr, zr) feeds the MLP; zeros past the end.  kIdx: grid point
-// job.idx[n] (a separate instantiation, so the dense kernel is the same code as without the indexed path)
-template <bool kIdx>
-__device__ __forceinline__ void point_of(const PointJob& job, int b, int64_t n, float& x, float& y, float& z, float& xr,
-                                         float& yr, float& zr) {
-  x = y = z = xr = yr = zr = 0.f;
-  if (n >= job.N) return;
-  if (job.pts) {
-    const float* q = job.pts + ((int64_t)b * job.N + n) * 3;
-    x = q[0]; y = q[1]; z = q[2];
-    if (job.pts_rot) {
-      const float* r = job.pts_rot + ((int64_t)b * job.N + n) * 3;
-      xr = r[0]; yr = r[1]; zr = r[2];
-    } else { xr = x; yr = y; zr = z; }
-  } else {
-    const int R = job.R;
-    const int64_t m = kIdx ? grid_index(job, n) : n;
-    const int ix = (int)(m % R);
-    const int64_t tt = m / R;
-    const int iy = (int)(tt % R);
-    const int iz = (int)(tt / R) + job.z0;
-    const float* ax = job.axes + (int64_t)b * 3 * R;
-    x = ax[ix]; y = ax[R + iy]; z = ax[2 * R + iz];
-    xr = x; yr = y; zr = z;
-  }
-}
-__device__ __forceinline__ void project(const PointJob& job, int b, float x, float y, float z, float& u, float& v) {
-  const float* T = job.trans_mat + b * 12;
-  const float q0 = fmaf(z, T[6], fmaf(y, T[3], x * T[0])) + T[9];
-  const float q1 = fmaf(z, T[7], fmaf(y, T[4], x * T[1])) + T[10];
-  const float q2 = fmaf(z, T[8], fmaf(y, T[5], x * T[2])) + T[11];
-  u = fminf(job.clamp_max, fmaxf(0.f, q0 / q2));
-  v = fminf(job.clamp_max, fmaxf(0.f, q1 / q2));
-}
 // bilinear taps of point n into the projected feature map (element offsets, -1 = outside; weights 0 there)
-template <bool kIdx>
 __device__ __forceinline__ void taps_of(const PointJob& job, int b, int64_t n, int (&off)[4], float (&wg)[4]) {
 #pragma unroll
   for (int k = 0; k < 4; ++k) { off[k] = -1; wg[k] = 0.f; }
@@ -123,8 +89,8 @@ __device__ __forceinline__ void taps_of(const PointJob& job, int b, int64_t n, i
     return;
   }
   float x, y, z, xr, yr, zr, u, v;
-  point_of<kIdx>(job, b, n, x, y, z, xr, yr, zr);
-  project(job, b, x, y, z, u, v);
+  point_of(job, b, n, x, y, z, xr, yr, zr);
+  project(job.trans_mat + b * 12, job.clamp_max, x, y, z, u, v);
   const int Wm = job.img_w, Hm = job.img_h;
   if (u > -1.f && v > -1.f && u < (float)Wm && v < (float)Hm) {
     const int fx = (int)floorf(u), fy = (int)floorf(v);
@@ -167,11 +133,8 @@ __device__ __forceinline__ void store_pair(uint8_t* xs, int row, int k, float a,
   }
 }
 
-// kCorr (MODE_F16F8): which correction products each tensor layer keeps -- bit 2l: (a - h(a)).w ("first"), bit 2l+1:
-//             a.(w - h(w)) ("second") for tensor layer l = 0..3 (fold1/conv2, fold1/conv3, fold2/conv1, fold2/conv2).
-//             0xFF = every correction; the shipped mask is CORR_DEFAULT.
 // the consumers hold two 64-register accumulators (plus the 32-register correction accumulator of MODE_F16F8)
-template <int kMode, int kCorr, bool kIdx>
+template <int kMode>
 __global__ void __launch_bounds__(NCONS, 1)
 point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint8_t* __restrict__ wpk,
                  int64_t tiles_per_img) {
@@ -180,7 +143,7 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
   __shared__ float part[2][2][PTS];            // fold2/conv5 partial sums [stream][warpgroup][point]
   __shared__ alignas(8) uint64_t full[NSLOT][2];   // [slot][consuming warpgroup]: half-stage landed
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  constexpr int kC = (kMode == MODE_F16F8) ? kCorr : 0;
+  constexpr int kC = (kMode == MODE_F16F8) ? CORR_DEFAULT : 0;
   const int64_t total_tiles = tiles_per_img * job.B;
   const int my_tiles =
       ((int64_t)blockIdx.x < total_tiles) ? (int)((total_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
@@ -226,10 +189,10 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
         const int p = tid >> 2, f0 = (tid & 3) * 16;
         const int64_t n = n0 + p;
         float x, y, z, xr, yr, zr;
-        point_of<kIdx>(job, b, n, x, y, z, xr, yr, zr);
+        point_of(job, b, n, x, y, z, xr, yr, zr);
         if (sx == 0 && (tid & 3) == 0 && job.out_uv && n < job.N) {
           float u, v;
-          project(job, b, x, y, z, u, v);
+          project(job.trans_mat + b * 12, job.clamp_max, x, y, z, u, v);
           float* o = job.out_uv + ((int64_t)b * job.N + n) * 2;
           o[0] = u; o[1] = v;
         }
@@ -324,8 +287,8 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
           int off[2][4];
           float wg[2][4];
           if (gather) {
-            taps_of<kIdx>(job, b, n0 + r0, off[0], wg[0]);
-            taps_of<kIdx>(job, b, n0 + r0 + 8, off[1], wg[1]);
+            taps_of(job, b, n0 + r0, off[0], wg[0]);
+            taps_of(job, b, n0 + r0 + 8, off[1], wg[1]);
           }
           const float* pm = job.pfeat ? job.pfeat : job.pmap + (int64_t)b * job.img_h * job.img_w * kHidden;
           const int sb = layer == 0 ? SB_B2 : (layer == 1 ? SB_B3 : SB_B4);
@@ -408,29 +371,32 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
   }
 }
 
-template <int kMode, int kCorr, bool kIdx>
+template <int kMode>
 int launch_var(disn_ctx* c, const PointJob& job, const SmallParams& sp, const void* wpk, int grid, int smem,
                int64_t tiles_per_img) {
   // the attribute belongs to (function, device): set per context, not per process (a second engine on another device
   // in the same process would otherwise launch with the 48 KB default)
-  auto key = (const void*)point_tc_kernel<kMode, kCorr, kIdx>;
+  auto key = (const void*)point_tc_kernel<kMode>;
   if (!c->attr_done.count(key)) {
-    DISN_CUDA_OK(cudaFuncSetAttribute(point_tc_kernel<kMode, kCorr, kIdx>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    DISN_CUDA_OK(cudaFuncSetAttribute(point_tc_kernel<kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     c->attr_done.insert(key);
   }
-  point_tc_kernel<kMode, kCorr, kIdx><<<grid, NCONS, smem, c->stream>>>(job, sp, reinterpret_cast<const uint8_t*>(wpk),
-                                                                           tiles_per_img);
+  point_tc_kernel<kMode><<<grid, NCONS, smem, c->stream>>>(job, sp, reinterpret_cast<const uint8_t*>(wpk), tiles_per_img);
   return 0;
 }
 
 }  // namespace
 
 // Pack both streams' tensor-core layers into the kernel's B-operand half-stage images, in consumption order:
-//   stream, layer, K slice t, 256-wide N block nb, half h (output features nb*256 + 128h + [0,128)):
-//   32 KB = [hi | lo] 16 KB bf16 SW128 tiles [128 rows n][64 k]
+//   stream, layer, K slice t, 256-wide N block nb, half h (output features nb*256 + 128h + [0,128)), 32 KB each:
+//   DISN_PREC_BF16X3  [hi | lo] 16 KB bf16 SW128 tiles [128 rows n][64 k];
+//   DISN_PREC_F16F8   [fp16 W, SW128, 16 KB | e5m2(w.2^-s1), SW64, 8 KB | e5m2((w - fp16(w)).2^s2), SW64, 8 KB].
+//   The exponents follow the layer's weight rms (2^L) so that the e5m2 operands (normal range 2^-14 .. 2^15,
+//   2 mantissa bits) sit mid-range for O(1) activations: s1 = 10 + L, s2 = 12 + L; the matching activation
+//   multipliers 2^s1 and 2^-s2 go to the kernel.
 int tc_pack_weights(disn_ctx* c) {
   const size_t total = (size_t)HS_PER_TILE * HS_BYTES;
-  std::vector<uint8_t> img(total, 0);
+  std::vector<uint8_t> img(total, 0), img8(total, 0);
   size_t stage = 0;
   for (int sidx = 0; sidx < 2; ++sidx) {
     const std::string p = sidx ? "sdfprediction_imgfeat" : "sdfprediction";
@@ -443,44 +409,6 @@ int tc_pack_weights(disn_ctx* c) {
       DISN_CUDA_OK(cudaMemcpyAsync(w.data(), it->second.ptr(), w.size() * sizeof(float), cudaMemcpyDeviceToHost,
                                    c->stream));
       DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
-      for (int t = 0; t < K / 64; ++t)
-        for (int nb = 0; nb < N / 256; ++nb, ++stage)
-          for (int half = 0; half < 2; ++half) {
-            const size_t pos = (size_t)sidx * STAGES_PER_STREAM + kLayerPos[layer] + (size_t)(t * (N / 256) + nb);
-            uint8_t* dst = img.data() + (2 * pos + half) * HS_BYTES;
-            for (int nl = 0; nl < 128; ++nl) {
-              const int n = nb * 256 + half * 128 + nl;
-              for (int k = 0; k < 64; ++k) {
-                const float v = w[(size_t)(t * 64 + k) * N + n];
-                const __nv_bfloat16 hi = __float2bfloat16(v);
-                const __nv_bfloat16 lo = __float2bfloat16(v - __bfloat162float(hi));
-                memcpy(dst + tc::sw128_offset(nl, k / 8) + (k % 8) * 2, &hi, 2);
-                memcpy(dst + W_TILE + tc::sw128_offset(nl, k / 8) + (k % 8) * 2, &lo, 2);
-              }
-            }
-          }
-    }
-  }
-  DISN_REQUIRE(stage == (size_t)2 * STAGES_PER_STREAM, "internal: stage count");
-  if (c->tc_weights.ensure(total) || c->tc_weights_f8.ensure(total)) return -1;
-  DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights.as<void>(), img.data(), total, cudaMemcpyHostToDevice, c->stream));
-  DISN_CUDA_OK(cudaStreamSynchronize(c->stream));   // ordered on the ctx stream (see conv_tc_pack)
-
-  // ---- DISN_PREC_F16F8 images: per half-stage: [fp16 W, SW128, 16 KB | e5m2(w.2^-s1), SW64, 8 KB |
-  //      e5m2((w - fp16(w)).2^s2), SW64, 8 KB].  The exponents follow the layer's weight rms (2^L) so that the
-  //      e5m2 operands (normal range 2^-14 .. 2^15, 2 mantissa bits) sit mid-range for O(1) activations:
-  //      s1 = 10 + L, s2 = 12 + L; the matching activation multipliers 2^s1 and 2^-s2 go to the kernel.
-  std::fill(img.begin(), img.end(), 0);
-  for (int sidx = 0; sidx < 2; ++sidx) {
-    const std::string p = sidx ? "sdfprediction_imgfeat" : "sdfprediction";
-    const char* names[4] = {"/fold1/conv2/weights", "/fold1/conv3/weights", "/fold2/conv1/weights", "/fold2/conv2/weights"};
-    for (int layer = 0; layer < 4; ++layer) {
-      auto it = c->weights.find(p + names[layer]);
-      const int K = layer_k(layer), N = layer_n(layer);
-      std::vector<float> w((size_t)K * N);
-      DISN_CUDA_OK(cudaMemcpyAsync(w.data(), it->second.ptr(), w.size() * sizeof(float), cudaMemcpyDeviceToHost,
-                                   c->stream));
-      DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
       double ss = 0;
       for (float v : w) ss += (double)v * v;
       const double rms = std::sqrt(ss / (double)w.size());
@@ -489,27 +417,36 @@ int tc_pack_weights(disn_ctx* c) {
       c->tc_act_scale[sidx][layer][0] = std::ldexp(1.f, s1);
       c->tc_act_scale[sidx][layer][1] = std::ldexp(1.f, -s2);
       for (int t = 0; t < K / 64; ++t)
-        for (int nb = 0; nb < N / 256; ++nb)
+        for (int nb = 0; nb < N / 256; ++nb, ++stage)
           for (int half = 0; half < 2; ++half) {
             const size_t pos = (size_t)sidx * STAGES_PER_STREAM + kLayerPos[layer] + (size_t)(t * (N / 256) + nb);
             uint8_t* dst = img.data() + (2 * pos + half) * HS_BYTES;
+            uint8_t* dst8 = img8.data() + (2 * pos + half) * HS_BYTES;
             for (int nl = 0; nl < 128; ++nl) {
               const int n = nb * 256 + half * 128 + nl;
               for (int k = 0; k < 64; ++k) {
                 const float v = w[(size_t)(t * 64 + k) * N + n];
+                const uint32_t o16 = tc::sw128_offset(nl, k / 8) + (k % 8) * 2;
+                const __nv_bfloat16 hi = __float2bfloat16(v);
+                const __nv_bfloat16 lo = __float2bfloat16(v - __bfloat162float(hi));
+                memcpy(dst + o16, &hi, 2);
+                memcpy(dst + W_TILE + o16, &lo, 2);
                 const __half hv = __float2half_rn(v);
-                memcpy(dst + tc::sw128_offset(nl, k / 8) + (k % 8) * 2, &hv, 2);
+                memcpy(dst8 + o16, &hv, 2);
                 const uint32_t o8 = tc::sw64_offset(nl, k / 16) + (k % 16);
-                dst[W_TILE + o8] = (uint8_t)__nv_cvt_float_to_fp8(std::ldexp(v, -s1), __NV_SATFINITE, __NV_E5M2);
-                dst[W_TILE + W8_TILE + o8] =
+                dst8[W_TILE + o8] = (uint8_t)__nv_cvt_float_to_fp8(std::ldexp(v, -s1), __NV_SATFINITE, __NV_E5M2);
+                dst8[W_TILE + W8_TILE + o8] =
                     (uint8_t)__nv_cvt_float_to_fp8(std::ldexp(v - __half2float(hv), s2), __NV_SATFINITE, __NV_E5M2);
               }
             }
           }
     }
   }
-  DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights_f8.as<void>(), img.data(), total, cudaMemcpyHostToDevice, c->stream));
-  DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
+  DISN_REQUIRE(stage == (size_t)2 * STAGES_PER_STREAM, "internal: stage count");
+  if (c->tc_weights.ensure(total) || c->tc_weights_f8.ensure(total)) return -1;
+  DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights.as<void>(), img.data(), total, cudaMemcpyHostToDevice, c->stream));
+  DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights_f8.as<void>(), img8.data(), total, cudaMemcpyHostToDevice, c->stream));
+  DISN_CUDA_OK(cudaStreamSynchronize(c->stream));   // ordered on the ctx stream (see conv_tc_pack)
 
   // host copy of the small per-stream parameters at the SB_* offsets (the kernel's __grid_constant__ parameter table)
   for (int sidx = 0; sidx < 2; ++sidx) {
@@ -543,26 +480,8 @@ int launch_point_tc(disn_ctx* c, const PointJob& job_in) {
   const int64_t total = tiles_per_img * job.B;
   if (total == 0) return 0;
   const int grid = (int)std::min<int64_t>(total, c->num_sms);
-  int corr = CORR_DEFAULT;
-  if (const char* e = getenv("DISN_TC_CORR")) corr = (int)strtol(e, nullptr, 0);      // A/B: 0xFF = every correction
-  int rc = -2;
-  const bool idx = job.idx != nullptr;
-  if (!f8) {
-    rc = idx ? launch_var<MODE_BF16X3, 0xFF, true>(c, job, sp, wpk, grid, smem, tiles_per_img)
-             : launch_var<MODE_BF16X3, 0xFF, false>(c, job, sp, wpk, grid, smem, tiles_per_img);
-  } else {
-    switch (corr) {
-      case 0xFF:
-        rc = idx ? launch_var<MODE_F16F8, 0xFF, true>(c, job, sp, wpk, grid, smem, tiles_per_img)
-                 : launch_var<MODE_F16F8, 0xFF, false>(c, job, sp, wpk, grid, smem, tiles_per_img);
-        break;
-      case 0xDF:
-        rc = idx ? launch_var<MODE_F16F8, 0xDF, true>(c, job, sp, wpk, grid, smem, tiles_per_img)
-                 : launch_var<MODE_F16F8, 0xDF, false>(c, job, sp, wpk, grid, smem, tiles_per_img);
-        break;
-      default: DISN_REQUIRE(false, "DISN_TC_CORR: only 0xFF (all corrections) and 0xDF (default) are built");
-    }
-  }
+  const int rc = f8 ? launch_var<MODE_F16F8>(c, job, sp, wpk, grid, smem, tiles_per_img)
+                    : launch_var<MODE_BF16X3>(c, job, sp, wpk, grid, smem, tiles_per_img);
   if (rc) return rc;
   c->launches++;
   DISN_CUDA_OK(cudaGetLastError());

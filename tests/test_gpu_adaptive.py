@@ -186,6 +186,15 @@ def test_errors(weights, engines, demo_img):
             eng.eval_grid_adaptive(BOX, tm, 16, band=band)
     with pytest.raises(DisnError, match="outside"):
         eng.eval_grid_indexed(BOX, tm, 16, [0, 17 ** 3])
+    # device indices are checked on the device: the call returns, the next synchronize() reports the bad index
+    import torch
+    d_idx = torch.tensor([0, 17 ** 3, 5], dtype=torch.int32, device="cuda:0")
+    d_tm = torch.from_numpy(np.ascontiguousarray(tm, np.float32)).to("cuda:0")
+    d_out = torch.empty(3, dtype=torch.float32, device="cuda:0")
+    torch.cuda.synchronize()
+    eng.eval_grid_indexed_device(BOX, d_tm.data_ptr(), 16, d_idx.data_ptr(), 3, d_out.data_ptr())
+    with pytest.raises(DisnError, match="outside"):
+        eng.synchronize()
     # band = +inf is valid and gives the dense grid; the context is still usable after the errors
     R = 65
     ptr, counts = eng.eval_grid_adaptive(BOX, tm, 64, band=np.inf)

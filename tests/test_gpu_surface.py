@@ -43,6 +43,10 @@ def test_intermediates_and_decoder_split_point(he_weights, precision):
         for got, key in ((pred, "pred_sdf"), (pg, "pred_sdf_value_global"), (pl_, "pred_sdf_value_local")):
             assert np.abs(got - ref[key]).max() / orc.SDF_WEIGHT <= 1e-4, key
         np.testing.assert_allclose(pg + pl_, pred, atol=1e-6)
+        # the decoder and the point kernels share one projection: the same uv, bit for bit
+        uv_dec = sess.engine.point_img_feat(pts, tm)[1]
+        uv_pts = sess.engine.eval_points(pts, tm, want_uv=True)[1]
+        np.testing.assert_array_equal(uv_dec.view(np.uint32), uv_pts.view(np.uint32))
         # get_decoder: feed the oracle's own features (float32 like a caller would) and compare with its decode
         emb = ref["img_embedding"].astype(np.float32).reshape(B, 1, 1, 1024)
         pf = ref["point_img_feat"].astype(np.float32)
