@@ -1,6 +1,6 @@
 // Diagnostics of the coarse-to-fine grid (adaptive.cu) and mesh (adaptive_mesh.cu), exported by libdisn_b200_test.so
-// only: the evaluated-point mask of the last grid, the refinement and the mesh with values read from a given dense field
-// instead of the network, the phase times, the mesher's buffer bytes and the edge ids of its vertices.
+// only: the evaluated-point mask of the last grid, both paths with the values of their one refinement read from a given
+// dense field instead of the network, the phase times, the mesher's buffer bytes and the edge ids of its vertices.
 #include <cmath>
 
 #include "../../include/disn_b200_test.h"

@@ -293,22 +293,21 @@ struct disn_ctx {
   disn::DevBuffer d_grid;
   disn::DevBuffer d_idx;        // host-index staging of disn_eval_grid_indexed
   disn::DevBuffer d_rows;       // eval_grid_points: x,y,z rows of one chunk of listed grid points
-  // coarse-to-fine grid (adaptive.cu): the filled grid, one byte per point (1 = evaluated), the block states of every
-  // level, the per-level index list and its values, compaction counts and scan scratch, host-field staging, the
-  // pinned level total and the phase events; ad_R / ad_levels describe the last call
-  disn::DevBuffer ad_grid, ad_mark, ad_state, ad_list, ad_vals, ad_chunk, ad_sums, ad_field;
+  // coarse-to-fine refinement (adaptive.cu), one set for the grid and the mesher: block states of every level, the coarse
+  // lattice values, each level's active blocks, the sort buffers of the level lists (the mesher's crossing cells reuse
+  // them), sort scratch, the network's value chunk, device counters with their pinned mirror
+  disn::DevBuffer ad_state, ad_coarse, ad_active[4], ad_keys[2], ad_sort_tmp, ad_vals, ad_cnt;
   disn::PinnedBuffer ad_host;
+  // coarse-to-fine grid (adaptive.cu): the filled grid, one byte per point (1 = evaluated), host-field staging and the
+  // phase events; ad_R / ad_levels describe the last call
+  disn::DevBuffer ad_grid, ad_mark, ad_field;
   cudaEvent_t ad_ev[7] = {};
   int32_t ad_R = 0, ad_levels = 0;
   disn::DevBuffer d_mc_in;
-  // coarse-to-fine mesh without a dense grid (adaptive_mesh.cu): block states of every level, the coarse lattice values,
-  // each level's active blocks and value table, the sort buffers of the level lists and then of the crossing cells, the
-  // crossing edges, the network's value chunk, cases and face offsets of the cells, scan scratch, device counters with
-  // their pinned mirror and the phase events.  am_nv: vertices of the last call (-1: none or failed), am_edges_sorted:
-  // its sorted crossing edges (vertex v = edge of rank v)
-  disn::DevBuffer am_state, am_coarse, am_active[4], am_table[4], am_keys[2], am_edges[2], am_sort_tmp, am_vals, am_case,
-      am_tri, am_sums, am_cnt;
-  disn::PinnedBuffer am_host;
+  // coarse-to-fine mesh without a dense grid (adaptive_mesh.cu): each level's value table, the crossing edges, cases and
+  // face offsets of the cells, scan scratch and the phase events.  am_nv: vertices of the last call (-1: none or failed),
+  // am_edges_sorted: its sorted crossing edges (vertex v = edge of rank v)
+  disn::DevBuffer am_table[4], am_edges[2], am_case, am_tri, am_sums;
   cudaEvent_t am_ev[4] = {};
   int64_t am_nv = -1;
   const unsigned long long* am_edges_sorted = nullptr;
@@ -379,7 +378,8 @@ int grid_axes(disn_ctx* c, const double* sdf_params, int B, int R);
 template <class Index>
 int eval_grid_points(disn_ctx* c, int image, int R, const float* d_tm, const Index* idx, int64_t n, float* out, int s = 1);
 // adaptive.cu: coarse-to-fine grid of one image; values come from `field` (device [R,R,R]) when it is non-null, else from
-// the network (eval_grid_points, with d_tm and the axis tables as above).  The filled grid stays in c->ad_grid.
+// the network (eval_grid_points, with d_tm and the axis tables as above).  The filled grid stays in c->ad_grid, the
+// evaluated-point marks in c->ad_mark.
 int adaptive_run(disn_ctx* c, const float* field, int image, const float* d_tm, int32_t res, const double* sdf_params,
                  float iso, double band, int64_t* level_counts, int32_t* n_levels);
 // adaptive_mesh.cu: the mesh of adaptive_run's grid followed by mc_run, built from the surface blocks alone (s0 >= 2);

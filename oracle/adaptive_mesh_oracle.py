@@ -18,53 +18,6 @@ from oracle import adaptive_oracle as ao
 from oracle import mc_oracle as mo
 
 
-def values(F, mask, states, res, z, y, x):
-    """Values of the dense adaptive grid at points (z, y, x): F where evaluated (mask), else the trilinear fill of the
-    finest classified inactive block, first candidate in (z, y, x) order (adaptive_oracle's fill rule)."""
-    z, y, x = (np.asarray(v, np.int64) for v in (z, y, x))
-    out = np.empty(len(z), np.float32)
-    ev = mask[z, y, x]
-    out[ev] = F[z[ev], y[ev], x[ev]]
-    todo = np.flatnonzero(~ev)
-    zz, yy, xx = z[todo], y[todo], x[todo]
-    done = np.zeros(len(todo), bool)
-    for s, st in reversed(states):
-        nb = res // s
-        cand = []
-        for c in (zz, yy, xx):
-            q0 = c // s
-            v0 = q0 < nb
-            v1 = (c % s == 0) & (q0 >= 1)
-            cand.append(((np.where(v0, q0, q0 - 1), q0 - 1), v0.astype(np.int64) + v1))
-        (cz, kz), (cy, ky), (cx, kx) = cand
-        for a in (0, 1):
-            for b in (0, 1):
-                for d in (0, 1):
-                    ok = ~done & (a < kz) & (b < ky) & (d < kx)
-                    if not ok.any():
-                        continue
-                    qz, qy, qx = cz[a][ok], cy[b][ok], cx[d][ok]
-                    hit = st[qz, qy, qx] == 1
-                    sel = np.flatnonzero(ok)[hit]
-                    if not len(sel):
-                        continue
-                    oz, oy, ox = qz[hit] * s, qy[hit] * s, qx[hit] * s
-                    inv = np.float32(1) / np.float32(s)
-                    tx = (xx[sel] - ox).astype(np.float32) * inv
-                    ty = (yy[sel] - oy).astype(np.float32) * inv
-                    tz = (zz[sel] - oz).astype(np.float32) * inv
-                    czv = []
-                    for kk in (0, 1):
-                        zk = oz + kk * s
-                        c0 = ao._lerp(tx, F[zk, oy, ox], F[zk, oy, ox + s])
-                        c1 = ao._lerp(tx, F[zk, oy + s, ox], F[zk, oy + s, ox + s])
-                        czv.append(ao._lerp(ty, c0, c1))
-                    out[todo[sel]] = ao._lerp(tz, czv[0], czv[1])
-                    done[sel] = True
-    assert done.all(), "a point outside every inactive block was never evaluated"
-    return out
-
-
 def _cells(block, s):
     return block.repeat(s, 0).repeat(s, 1).repeat(s, 2)
 
@@ -117,7 +70,7 @@ def mesh(field, sdf_params, iso: float = 0.0, band: float = 1.0, rule_ii: bool =
     iso32 = np.float32(iso)
     case = np.zeros(len(cz), np.int64)
     for k in range(8):
-        v = values(F, mask, states, res, cz + (k >> 2 & 1), cy + (k >> 1 & 1), cx + (k & 1))
+        v = ao.values(F, mask, states, res, cz + (k >> 2 & 1), cy + (k >> 1 & 1), cx + (k & 1))
         case |= (v < iso32).astype(np.int64) << k
     nt = mo.NTRI[case]
     keep = nt > 0
@@ -132,8 +85,8 @@ def mesh(field, sdf_params, iso: float = 0.0, band: float = 1.0, rule_ii: bool =
     a = E % 3
     q = E // 3
     x, y, z = q % R, (q // R) % R, q // (R * R)
-    v0 = values(F, mask, states, res, z, y, x).astype(np.float64)
-    v1 = values(F, mask, states, res, z + (a == 2), y + (a == 1), x + (a == 0)).astype(np.float64)
+    v0 = ao.values(F, mask, states, res, z, y, x).astype(np.float64)
+    v1 = ao.values(F, mask, states, res, z + (a == 2), y + (a == 1), x + (a == 0)).astype(np.float64)
     lo = np.asarray(sdf_params[:3], np.float64)
     h = (np.asarray(sdf_params[3:], np.float64) - lo) / np.float64(R - 1)
     t = (np.float64(iso32) - v0) / (v1 - v0)

@@ -1,7 +1,8 @@
 """NumPy twin of the coarse-to-fine SDF grid (disn_b200/csrc/adaptive.cu, DESIGN.md §4.9).
 
 Given the dense float32 field the network would produce, `refine` returns what the device computes: which points are
-evaluated, how many per level, and the filled grid, bit for bit.  Definitions (shared with the kernel):
+evaluated, how many per level, and the filled grid, bit for bit.  `values` is the fill rule at any set of points; the
+mesher's twin (oracle/adaptive_mesh_oracle.py) reads its cell corners with it.  Definitions (shared with the kernel):
   * s0 = the largest power of two <= 16 that divides res; s0 = 1 gives the dense grid.  The stride-s0 lattice is
     evaluated first, then levels s = s0, s0/2, ..., 2;
   * level s classifies the blocks of size s (closed cubes of lattice points, origin a multiple of s): all blocks at the
@@ -95,20 +96,29 @@ def refine(field, sdf_params, iso: float = 0.0, band: float = 1.0, want_states: 
         states.append((s, st))
         parent = st
         s //= 2
-    out = np.where(mask, F, np.float32(np.nan)).astype(np.float32)
-    flat = np.flatnonzero(~mask)
-    z, y, x = (v.astype(np.int64) for v in np.unravel_index(flat, F.shape))
-    done = np.zeros(len(flat), bool)
-    vals = np.zeros(len(flat), np.float32)
+    z, y, x = np.unravel_index(np.arange(F.size), F.shape)
+    out = values(F, mask, states, res, z, y, x).reshape(F.shape)
+    return (mask, counts, out, states) if want_states else (mask, counts, out)
+
+
+def values(F, mask, states, res, z, y, x):
+    """Values of the dense adaptive grid at points (z, y, x): F where evaluated (mask), else the trilinear fill of the
+    finest classified inactive block, first candidate in (z, y, x) order (the fill rule)."""
+    z, y, x = (np.asarray(v, np.int64) for v in (z, y, x))
+    out = np.empty(len(z), np.float32)
+    ev = mask[z, y, x]
+    out[ev] = F[z[ev], y[ev], x[ev]]
+    todo = np.flatnonzero(~ev)
+    zz, yy, xx = z[todo], y[todo], x[todo]
+    done = np.zeros(len(todo), bool)
     for s, st in reversed(states):                 # finest level first
         nb = res // s
         cand = []
-        for c in (z, y, x):
+        for c in (zz, yy, xx):
             q0 = c // s
             v0 = q0 < nb
             v1 = (c % s == 0) & (q0 >= 1)
-            first = np.where(v0, q0, q0 - 1)
-            cand.append(((first, q0 - 1), v0.astype(np.int64) + v1))
+            cand.append(((np.where(v0, q0, q0 - 1), q0 - 1), v0.astype(np.int64) + v1))
         (cz, kz), (cy, ky), (cx, kx) = cand
         for a in (0, 1):
             for b in (0, 1):
@@ -123,17 +133,16 @@ def refine(field, sdf_params, iso: float = 0.0, band: float = 1.0, want_states: 
                         continue
                     oz, oy, ox = qz[hit] * s, qy[hit] * s, qx[hit] * s
                     inv = np.float32(1) / np.float32(s)
-                    tx = (x[sel] - ox).astype(np.float32) * inv
-                    ty = (y[sel] - oy).astype(np.float32) * inv
-                    tz = (z[sel] - oz).astype(np.float32) * inv
+                    tx = (xx[sel] - ox).astype(np.float32) * inv
+                    ty = (yy[sel] - oy).astype(np.float32) * inv
+                    tz = (zz[sel] - oz).astype(np.float32) * inv
                     czv = []
                     for kk in (0, 1):
-                        zz = oz + kk * s
-                        c0 = _lerp(tx, F[zz, oy, ox], F[zz, oy, ox + s])
-                        c1 = _lerp(tx, F[zz, oy + s, ox], F[zz, oy + s, ox + s])
+                        zk = oz + kk * s
+                        c0 = _lerp(tx, F[zk, oy, ox], F[zk, oy, ox + s])
+                        c1 = _lerp(tx, F[zk, oy + s, ox], F[zk, oy + s, ox + s])
                         czv.append(_lerp(ty, c0, c1))
-                    vals[sel] = _lerp(tz, czv[0], czv[1])
+                    out[todo[sel]] = _lerp(tz, czv[0], czv[1])
                     done[sel] = True
     assert done.all(), "a point outside every inactive block was never evaluated"
-    out.reshape(-1)[flat] = vals
-    return (mask, counts, out, states) if want_states else (mask, counts, out)
+    return out
