@@ -21,9 +21,11 @@
 //   * weights are pre-split and pre-swizzled on the host into the exact shared-memory images of the B operand
 //     (32 KB per 128 output features x 64 k), packed in consumption order and streamed by the bulk-copy engine
 //     (cp.async.bulk) through a 3-slot mbarrier ring.  Half-stages alternate between the two warpgroups, so each
-//     (slot, warpgroup) has its own "landed" barrier and every barrier phase has one waiter; the warpgroup that has
-//     just finished half-stage g refills its slot with half-stage g + 3 (no separate producer warp: the register file
-//     is allocated to warps in groups of four, and the consumers need all of it);
+//     (slot, warpgroup) has its own "landed" and "empty" barrier and every barrier phase has one waiter.  A warpgroup
+//     issues all MMAs of a half-stage as one commit group and waits for it once; each of its warps then arrives on the
+//     slot's empty barrier, and its first thread refills the slot with half-stage g + 3 when all four have (no
+//     separate producer warp: the register file is allocated to warps in groups of four, and the consumers need all
+//     of it);
 //   * the small per-stream parameters (biases, fold1/conv1, fold2/conv5) are a __grid_constant__ kernel parameter
 //     (constant bank, warp-uniform indexed loads).
 #include <algorithm>
@@ -133,7 +135,7 @@ __device__ __forceinline__ void store_pair(uint8_t* xs, int row, int k, float a,
   }
 }
 
-// the consumers hold two 64-register accumulators (plus the 32-register correction accumulator of MODE_F16F8)
+// the consumers hold two 64-register accumulators (plus the 64-register correction accumulator of MODE_F16F8)
 template <int kMode>
 __global__ void __launch_bounds__(NCONS, 1)
 point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint8_t* __restrict__ wpk,
@@ -142,6 +144,7 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
   TcSmem& s = *reinterpret_cast<TcSmem*>(smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u));
   __shared__ float part[2][2][PTS];            // fold2/conv5 partial sums [stream][warpgroup][point]
   __shared__ alignas(8) uint64_t full[NSLOT][2];   // [slot][consuming warpgroup]: half-stage landed
+  __shared__ alignas(8) uint64_t empty[NSLOT][2];  // [slot][consuming warpgroup]: its four warps are done reading it
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr int kC = (kMode == MODE_F16F8) ? CORR_DEFAULT : 0;
   const int64_t total_tiles = tiles_per_img * job.B;
@@ -152,6 +155,8 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
     for (int i = 0; i < NSLOT; ++i) {
       tc::mbar_init(&full[i][0], 1);
       tc::mbar_init(&full[i][1], 1);
+      tc::mbar_init(&empty[i][0], 4);
+      tc::mbar_init(&empty[i][1], 4);
     }
     tc::fence_barrier_init();
   }
@@ -176,7 +181,7 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
   uint32_t ph = 0;                               // phase bit per slot of full[slot][h]
   __half2 amax = __float2half2_rn(0.f);          // running maximum of this thread's fp16 A-operand values (MODE_F16F8)
   float acc[2][64];
-  float tmp[32];                                 // MODE_F16F8: corrections of one K slice, 64 columns
+  float tmp[64];                                 // MODE_F16F8: corrections of one half-stage
 
   for (int it = 0; it < my_tiles; ++it) {
     const int64_t tile = (int64_t)blockIdx.x + (int64_t)it * gridDim.x;
@@ -223,11 +228,12 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
 #pragma unroll
           for (int nb = 0; nb < 2; ++nb) {
             if (nb >= nnb) continue;
-            const uint32_t slot = g % NSLOT;
-            tc::mbar_wait(&full[slot][h], (ph >> slot) & 1u);
+            const uint32_t slot = g % NSLOT, par = (ph >> slot) & 1u;
+            tc::mbar_wait(&full[slot][h], par);
             ph ^= 1u << slot;
             const uint32_t xa = x_base + (uint32_t)t * X_SLICE, wb = w_base + slot * HS_BYTES;
             tc::acc_fence(acc[nb]);
+            if constexpr (kMode == MODE_F16F8) tc::acc_fence(tmp);
             tc::wgmma_fence();
             if constexpr (kMode == MODE_BF16X3) {
 #pragma unroll
@@ -239,44 +245,43 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
 #pragma unroll
               for (int k = 0; k < 4; ++k)
                 tc::wgmma_m64n128<tc::KIND_BF16>(acc[nb], tc::desc_sw128(xa + 32u * k), tc::desc_sw128(wb + W_TILE + 32u * k), 1u);
-              tc::wgmma_commit();
-              tc::wgmma_wait<0>();
-              tc::acc_fence(acc[nb]);
             } else {
 #pragma unroll
               for (int k = 0; k < 4; ++k)
                 tc::wgmma_m64n128<tc::KIND_F16>(acc[nb], tc::desc_sw128(xa + 32u * k), tc::desc_sw128(wb + 32u * k), (t | k) ? 1u : 0u);
-              tc::wgmma_commit();
-              // corrections in two 64-column chunks through a zero-initialised accumulator, added in fp32
+              // corrections into the zero-initialised side accumulator, in the same commit group; they are added after
+              // the wait, so each element still gets main(t), then + corr(t), then main(t + 1)
+              if (k1) {
 #pragma unroll
-              for (int ch = 0; ch < 2; ++ch) {
-                if (!(k1 || k2)) break;
-                const uint32_t wc = wb + W_TILE + (uint32_t)ch * (W8_TILE / 2);   // rows 64ch.. of the SW64 B tiles
-                tc::acc_fence(tmp);
-                tc::wgmma_fence();
-                if (k1) {
-#pragma unroll
-                  for (int k = 0; k < 2; ++k)
-                    tc::wgmma_m64n64_e5m2(tmp, tc::desc_sw64(xa + X_TILE + 32u * k), tc::desc_sw64(wc + 32u * k), k ? 1u : 0u);
-                }
-                if (k2) {
-#pragma unroll
-                  for (int k = 0; k < 2; ++k)
-                    tc::wgmma_m64n64_e5m2(tmp, tc::desc_sw64(xa + X_TILE + X8_TILE + 32u * k), tc::desc_sw64(wc + W8_TILE + 32u * k),
-                                          (k1 || k) ? 1u : 0u);
-                }
-                tc::wgmma_commit();
-                tc::wgmma_wait<0>();
-                tc::acc_fence(tmp);
-                tc::acc_fence(acc[nb]);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) acc[nb][32 * ch + i] += tmp[i];
+                for (int k = 0; k < 2; ++k)
+                  tc::wgmma_m64n128<tc::KIND_E5M2>(tmp, tc::desc_sw64(xa + X_TILE + 32u * k), tc::desc_sw64(wb + W_TILE + 32u * k),
+                                                   k ? 1u : 0u);
               }
-              tc::wgmma_wait<0>();
-              tc::acc_fence(acc[nb]);
+              if (k2) {
+#pragma unroll
+                for (int k = 0; k < 2; ++k)
+                  tc::wgmma_m64n128<tc::KIND_E5M2>(tmp, tc::desc_sw64(xa + X_TILE + X8_TILE + 32u * k),
+                                                   tc::desc_sw64(wb + W_TILE + W8_TILE + 32u * k), (k1 || k) ? 1u : 0u);
+              }
             }
-            named_bar_sync(2 + h, 128);         // every warp of this warpgroup is done with the slot
-            if ((tid & 127) == 0 && g + NSLOT < total_hs) load_stage(g + NSLOT);
+            tc::wgmma_commit();
+            tc::wgmma_wait<0>();
+            tc::acc_fence(acc[nb]);
+            // this warp is done with the slot; the warpgroup's first thread refills it once all four warps are.  The
+            // other warps arrive without waiting on anything, so that wait always completes.
+            const bool refill = g + NSLOT < total_hs;
+            if (refill && lane == 0) tc::mbar_arrive(&empty[slot][h]);
+            if constexpr (kMode == MODE_F16F8) {
+              if (k1 || k2) {
+                tc::acc_fence(tmp);
+#pragma unroll
+                for (int i = 0; i < 64; ++i) acc[nb][i] += tmp[i];
+              }
+            }
+            if (refill && (tid & 127) == 0) {
+              tc::mbar_wait(&empty[slot][h], par);
+              load_stage(g + NSLOT);
+            }
             g += 2;
           }
         }
@@ -294,12 +299,18 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
           const int sb = layer == 0 ? SB_B2 : (layer == 1 ? SB_B3 : SB_B4);
           const float* gb = (sx == 0 && layer == 2) ? job.gbias + (int64_t)b * kHidden : nullptr;
           const float sc_lo = job.act_scale[sx][layer + 1][0], sc_hi = job.act_scale[sx][layer + 1][1];
+          // MODE_F16F8: the thread's row and column bases, made opaque here so that the epilogue's ~100 store offsets are
+          // derived from them in place: the compiler would otherwise hoist them out of the tile loop and keep them live
+          // across the MMA loops next to the main and side accumulators, where they spill.  MODE_BF16X3 has the
+          // registers to keep them, and recomputing them costs it time.
+          int row = r0, cbase = h * 128 + cq;
+          if constexpr (kMode == MODE_F16F8) asm volatile("" : "+r"(row), "+r"(cbase));
 #pragma unroll
           for (int nb = 0; nb < 2; ++nb) {
             if (nb >= nnb) continue;
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
-              const int col = nb * 256 + h * 128 + 8 * j + cq;
+              const int col = nb * 256 + cbase + 8 * j;
               float bias[2];
               if (gb) { bias[0] = gb[col]; bias[1] = gb[col + 1]; }
               else { bias[0] = sp.v[sx][sb + col]; bias[1] = sp.v[sx][sb + col + 1]; }
@@ -320,7 +331,7 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
                 }
                 const float va = fmaxf(acc[nb][4 * j + 2 * e2] + v2[0], 0.f);
                 const float vb = fmaxf(acc[nb][4 * j + 2 * e2 + 1] + v2[1], 0.f);
-                store_pair<kMode>(s.x[col >> 6], r0 + 8 * e2, col & 63, va, vb, sc_lo, sc_hi, amax);
+                store_pair<kMode>(s.x[col >> 6], row + 8 * e2, col & 63, va, vb, sc_lo, sc_hi, amax);
               }
             }
           }
