@@ -100,6 +100,7 @@ TEST_EXPORTS = {
     "disn_tc_selftest": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "disn_tc_selftest_mixed": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                          C.c_void_p, C.c_void_p]),
+    "disn_debug_tc_weights": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     "disn_adaptive_mask": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
     "disn_adaptive_from_field": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_float, C.c_double,
                                            C.c_uint32, C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_int32)]),

@@ -26,6 +26,11 @@ int disn_tc_stream_probe(int device);
 /* Diagnostic: prints the issue cost (cycles) of the mbarrier / wgmma synchronisation instructions of the consumers. */
 int disn_tc_op_probe(int device);
 
+/* Diagnostic of the tensor-core point kernel: the packed weight image of operand mode `precision` (DISN_PREC_BF16X3 or
+ * DISN_PREC_F16F8) -> image[nbytes] (host; nbytes must be the packed size, 132 half-stages of 32 KB in consumption order,
+ * see tc_pack_weights) and the e5m2 activation multipliers [stream][layer]{(a - h(a)) scale, a scale} -> act_scale[16]. */
+int disn_debug_tc_weights(disn_ctx* ctx, int32_t precision, int64_t nbytes, uint8_t* image, float* act_scale);
+
 /* Diagnostics of the coarse-to-fine grid (disn_eval_grid_adaptive):
  *   disn_adaptive_mask: points [first, first + n) of the last call's evaluated-point mask -> out uint8[n] (1 = evaluated);
  *   disn_adaptive_from_field: the same refinement with values read from field [R,R,R] (host, or device with
