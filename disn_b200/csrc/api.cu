@@ -185,6 +185,11 @@ int disn_finalize_weights(disn_ctx* c) {
     if (check_shape(c, p + "/fold2/conv5/weights", {256, 1})) return -2;
     for (const char* l : {"fold1/conv1", "fold1/conv2", "fold1/conv3", "fold2/conv1", "fold2/conv2", "fold2/conv5"})
       DISN_REQUIRE(c->weights.count(p + "/" + l + "/biases"), "missing variable " + p + "/" + l + "/biases");
+    // the point kernels read these biases by output feature straight from the tensors
+    const struct { const char* l; int64_t n; } widths[5] = {
+        {"fold1/conv1", 64}, {"fold1/conv2", 256}, {"fold1/conv3", 512}, {"fold2/conv1", 512}, {"fold2/conv2", 256}};
+    for (const auto& e : widths)
+      DISN_REQUIRE(c->weights.at(p + "/" + e.l + "/biases").numel == e.n, "mis-shaped variable " + p + "/" + e.l + "/biases");
   }
   if (tc_pack_weights(c)) return -1;
   c->weights_dirty = false;

@@ -259,7 +259,6 @@ struct disn_ctx {
   disn::DevBuffer tc_weights;          // bf16 hi/lo stage images of the point MLP (DISN_PREC_BF16X3)
   disn::DevBuffer tc_weights_f8;       // fp16 + e5m2 stage images (DISN_PREC_F16F8)
   float tc_act_scale[2][4][2] = {};
-  float tc_small[2][2048] = {};         // host copy of the per-stream small parameters (the point kernel's __grid_constant__ table)
   std::map<std::string, disn::DevBuffer> enc_tc_weights;   // packed bf16 hi/lo stage images of the encoder GEMMs
   // marching cubes: persistent scratch + the device-resident mesh of the last run (mc.cu)
   disn::DevBuffer mc_code, mc_vbase, mc_chunk, mc_sums, mc_totals;

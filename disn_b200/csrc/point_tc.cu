@@ -26,8 +26,8 @@
 //     slot's empty barrier, and its first thread refills the slot with half-stage g + 3 when all four have (no
 //     separate producer warp: the register file is allocated to warps in groups of four, and the consumers need all
 //     of it);
-//   * the small per-stream parameters (biases, fold1/conv1, fold2/conv5) are a __grid_constant__ kernel parameter
-//     (constant bank, warp-uniform indexed loads).
+//   * the small per-stream parameters (biases, fold1/conv1, fold2/conv5) are read from global memory through the
+//     read-only cache: the lanes of a warp read different features, and the constant bank would serialise them.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -58,8 +58,6 @@ constexpr int HS_PER_TILE = 2 * 2 * STAGES_PER_STREAM;
 // fold2/conv2): bit 2l (a - h(a)).w ("first"), bit 2l+1 a.(w - h(w)) ("second").  Every correction except the second
 // product of fold2/conv1 (DESIGN.md section 3).
 constexpr int CORR_DEFAULT = 0xDF;
-// shared-memory table of small fp32 parameters per stream
-constexpr int SB_B2 = 0, SB_B3 = 256, SB_B4 = 768, SB_B5 = 1280, SB_W6 = 1536, SB_W1 = 1792, SB_B1 = 1984, SB_STRIDE = 2048;
 __host__ __device__ constexpr int layer_k(int l) { return l == 0 ? 64 : (l == 1 ? 256 : 512); }
 __host__ __device__ constexpr int layer_n(int l) { return (l == 1 || l == 2) ? 512 : 256; }
 constexpr int kLayerPos[4] = {0, 1, 9, 25};   // first stage of each tensor layer within a stream
@@ -68,8 +66,6 @@ constexpr int kLayerPos[4] = {0, 1, 9, 25};   // first stage of each tensor laye
 constexpr int MODE_BF16X3 = 0;   // x = hi + lo (bf16): hi*hi + lo*hi + hi*lo, 12 MMAs per 64-wide K slice
 constexpr int MODE_F16F8 = 1;    // fp16 main product + two e5m2 correction products:
                                  //   a.w ~= h(a).h(w) + e((a-h(a)).2^s1).e(w.2^-s1) + e(a.2^-s2).e((w-h(w)).2^s2), 4 + 2 + 2 MMAs
-
-struct SmallParams { float v[2][SB_STRIDE]; };   // per stream: b2 b3 b4 b5 w6 w1 b1 at the SB_* offsets
 
 struct TcSmem {
   alignas(1024) uint8_t w[NSLOT][HS_BYTES];     // weight ring                                  96 KB
@@ -138,7 +134,7 @@ __device__ __forceinline__ void store_pair(uint8_t* xs, int row, int k, float a,
 // the consumers hold two 64-register accumulators (plus the 64-register correction accumulator of MODE_F16F8)
 template <int kMode>
 __global__ void __launch_bounds__(NCONS, 1)
-point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint8_t* __restrict__ wpk,
+point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
                  int64_t tiles_per_img) {
   extern __shared__ uint8_t smem_raw[];
   TcSmem& s = *reinterpret_cast<TcSmem*>(smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u));
@@ -201,16 +197,20 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
           float* o = job.out_uv + ((int64_t)b * job.N + n) * 2;
           o[0] = u; o[1] = v;
         }
+        const StreamWeights& sw = sx ? job.l : job.g;
 #pragma unroll
         for (int j = 0; j < 16; j += 2) {
+          const float2 b1 = __ldg(reinterpret_cast<const float2*>(sw.b1 + f0 + j));
+          const float2 wx = __ldg(reinterpret_cast<const float2*>(sw.w1 + f0 + j));
+          const float2 wy = __ldg(reinterpret_cast<const float2*>(sw.w1 + 64 + f0 + j));
+          const float2 wz = __ldg(reinterpret_cast<const float2*>(sw.w1 + 128 + f0 + j));
           float v2[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int f = f0 + j + e;
-            float a = sp.v[sx][SB_B1 + f];
-            a = fmaf(xr, sp.v[sx][SB_W1 + f], a);
-            a = fmaf(yr, sp.v[sx][SB_W1 + 64 + f], a);
-            a = fmaf(zr, sp.v[sx][SB_W1 + 128 + f], a);
+            float a = e ? b1.y : b1.x;
+            a = fmaf(xr, e ? wx.y : wx.x, a);
+            a = fmaf(yr, e ? wy.y : wy.x, a);
+            a = fmaf(zr, e ? wz.y : wz.x, a);
             v2[e] = fmaxf(a, 0.f);
           }
           store_pair<kMode>(s.x[0], p, f0 + j, v2[0], v2[1], job.act_scale[sx][0][0], job.act_scale[sx][0][1], amax);
@@ -294,10 +294,13 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
           if (gather) {
             taps_of(job, b, n0 + r0, off[0], wg[0]);
             taps_of(job, b, n0 + r0 + 8, off[1], wg[1]);
+          } else {   // layer 2 of the global stream loads the taps too (see below), and drops them
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { off[k >> 2][k & 3] = -1; wg[k >> 2][k & 3] = 0.f; }
           }
           const float* pm = job.pfeat ? job.pfeat : job.pmap + (int64_t)b * job.img_h * job.img_w * kHidden;
-          const int sb = layer == 0 ? SB_B2 : (layer == 1 ? SB_B3 : SB_B4);
-          const float* gb = (sx == 0 && layer == 2) ? job.gbias + (int64_t)b * kHidden : nullptr;
+          const StreamWeights& sw = sx ? job.l : job.g;
+          const float* bias_v = layer == 0 ? sw.b2 : (layer == 1 ? sw.b3 : (sx == 0 ? job.gbias + (int64_t)b * kHidden : sw.b4));
           const float sc_lo = job.act_scale[sx][layer + 1][0], sc_hi = job.act_scale[sx][layer + 1][1];
           // MODE_F16F8: the thread's row and column bases, made opaque here so that the epilogue's ~100 store offsets are
           // derived from them in place: the compiler would otherwise hoist them out of the tile loop and keep them live
@@ -311,13 +314,15 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
               const int col = nb * 256 + cbase + 8 * j;
-              float bias[2];
-              if (gb) { bias[0] = gb[col]; bias[1] = gb[col + 1]; }
-              else { bias[0] = sp.v[sx][sb + col]; bias[1] = sp.v[sx][sb + col + 1]; }
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(bias_v + col));
+              const float bias[2] = {bb.x, bb.y};
 #pragma unroll
               for (int e2 = 0; e2 < 2; ++e2) {
                 float v2[2] = {bias[0], bias[1]};
-                if (gather) {
+                // layer 2 shares its code between the streams: the tap loads stay unconditional (every address is valid)
+                // so that the compiler can issue them ahead across j; a branch around them per j serialised their L2
+                // round trips.  Only the local stream adds the result.
+                if (layer == 2) {
                   float2 a = make_float2(0.f, 0.f);
 #pragma unroll
                   for (int k = 0; k < 4; ++k) {
@@ -326,8 +331,10 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
                     a.x = fmaf(wg[e2][k], m.x, a.x);
                     a.y = fmaf(wg[e2][k], m.y, a.y);
                   }
-                  v2[0] += a.x;
-                  v2[1] += a.y;
+                  if (gather) {
+                    v2[0] += a.x;
+                    v2[1] += a.y;
+                  }
                 }
                 const float va = fmaxf(acc[nb][4 * j + 2 * e2] + v2[0], 0.f);
                 const float vb = fmaxf(acc[nb][4 * j + 2 * e2 + 1] + v2[1], 0.f);
@@ -340,14 +347,16 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
         } else {
           // ---- fold2/conv2 output (256) -> ReLU -> fold2/conv5 dot product
           float pr[2] = {0.f, 0.f};
+          const StreamWeights& sw = sx ? job.l : job.g;
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const int col = h * 128 + 8 * j + cq;
+            const float2 b5 = __ldg(reinterpret_cast<const float2*>(sw.b5 + col));
+            const float2 w6 = __ldg(reinterpret_cast<const float2*>(sw.w6 + col));
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-              const int c = col + (e & 1);
-              const float a = fmaxf(acc[0][4 * j + e] + sp.v[sx][SB_B5 + c], 0.f);
-              pr[e >> 1] = fmaf(a, sp.v[sx][SB_W6 + c], pr[e >> 1]);
+              const float a = fmaxf(acc[0][4 * j + e] + ((e & 1) ? b5.y : b5.x), 0.f);
+              pr[e >> 1] = fmaf(a, (e & 1) ? w6.y : w6.x, pr[e >> 1]);
             }
           }
 #pragma unroll
@@ -383,7 +392,7 @@ point_tc_kernel(PointJob job, const __grid_constant__ SmallParams sp, const uint
 }
 
 template <int kMode>
-int launch_var(disn_ctx* c, const PointJob& job, const SmallParams& sp, const void* wpk, int grid, int smem,
+int launch_var(disn_ctx* c, const PointJob& job, const void* wpk, int grid, int smem,
                int64_t tiles_per_img) {
   // the attribute belongs to (function, device): set per context, not per process (a second engine on another device
   // in the same process would otherwise launch with the 48 KB default)
@@ -392,7 +401,7 @@ int launch_var(disn_ctx* c, const PointJob& job, const SmallParams& sp, const vo
     DISN_CUDA_OK(cudaFuncSetAttribute(point_tc_kernel<kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     c->attr_done.insert(key);
   }
-  point_tc_kernel<kMode><<<grid, NCONS, smem, c->stream>>>(job, sp, reinterpret_cast<const uint8_t*>(wpk), tiles_per_img);
+  point_tc_kernel<kMode><<<grid, NCONS, smem, c->stream>>>(job, reinterpret_cast<const uint8_t*>(wpk), tiles_per_img);
   return 0;
 }
 
@@ -458,22 +467,6 @@ int tc_pack_weights(disn_ctx* c) {
   DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights.as<void>(), img.data(), total, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaMemcpyAsync(c->tc_weights_f8.as<void>(), img8.data(), total, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));   // ordered on the ctx stream (see conv_tc_pack)
-
-  // host copy of the small per-stream parameters at the SB_* offsets (the kernel's __grid_constant__ parameter table)
-  for (int sidx = 0; sidx < 2; ++sidx) {
-    const std::string p = sidx ? "sdfprediction_imgfeat" : "sdfprediction";
-    const struct { const char* name; int off, n; } small[7] = {
-        {"/fold1/conv2/biases", SB_B2, 256}, {"/fold1/conv3/biases", SB_B3, 512}, {"/fold2/conv1/biases", SB_B4, 512},
-        {"/fold2/conv2/biases", SB_B5, 256}, {"/fold2/conv5/weights", SB_W6, 256}, {"/fold1/conv1/weights", SB_W1, 192},
-        {"/fold1/conv1/biases", SB_B1, 64}};
-    for (const auto& e : small) {
-      auto it = c->weights.find(p + e.name);
-      DISN_REQUIRE(it != c->weights.end() && it->second.numel == e.n, "missing or mis-shaped variable " + p + e.name);
-      DISN_CUDA_OK(cudaMemcpyAsync(&c->tc_small[sidx][e.off], it->second.ptr(), (size_t)e.n * sizeof(float),
-                                   cudaMemcpyDeviceToHost, c->stream));
-    }
-  }
-  DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
   return 0;
 }
 
@@ -481,18 +474,15 @@ int launch_point_tc(disn_ctx* c, const PointJob& job_in) {
   const bool f8 = c->cfg.precision == DISN_PREC_F16F8;
   const void* wpk = (f8 ? c->tc_weights_f8 : c->tc_weights).as<void>();
   DISN_REQUIRE(wpk != nullptr, "tensor-core weights not packed (call disn_finalize_weights)");
-  static_assert(sizeof(SmallParams) == sizeof(c->tc_small), "small-parameter table layout");
   PointJob job = job_in;
   memcpy(job.act_scale, c->tc_act_scale, sizeof(job.act_scale));
-  SmallParams sp;
-  memcpy(&sp, c->tc_small, sizeof(sp));
   const int smem = (int)sizeof(TcSmem) + 1024;
   const int64_t tiles_per_img = (job.N + PTS - 1) / PTS;
   const int64_t total = tiles_per_img * job.B;
   if (total == 0) return 0;
   const int grid = (int)std::min<int64_t>(total, c->num_sms);
-  const int rc = f8 ? launch_var<MODE_F16F8>(c, job, sp, wpk, grid, smem, tiles_per_img)
-                    : launch_var<MODE_BF16X3>(c, job, sp, wpk, grid, smem, tiles_per_img);
+  const int rc = f8 ? launch_var<MODE_F16F8>(c, job, wpk, grid, smem, tiles_per_img)
+                    : launch_var<MODE_BF16X3>(c, job, wpk, grid, smem, tiles_per_img);
   if (rc) return rc;
   c->launches++;
   DISN_CUDA_OK(cudaGetLastError());
