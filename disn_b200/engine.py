@@ -583,6 +583,31 @@ class Engine:
         val = inter.value / uni.value if uni.value else float("nan")
         return (val, inter.value, uni.value, o1, o2) if want_grids else val
 
+    def iou_views(self, ref_verts, ref_faces, views, dim: int = 110, want_grids: bool = False):
+        """iou_pymesh (test/test_iou.py:208-233) of one reference mesh against every mesh of `views`, a list of
+        (verts, faces), in one call (disn_iou_views): the reference is voxelised once.  Returns (iou [V] float64,
+        intersection [V] int64, union [V] int64), plus the occupancy grids [V+1,dim,dim,dim] uint8 (the reference's
+        first) when want_grids.  iou[v] is intersection / union, NaN when the union is empty."""
+        rv, rf = _f32(ref_verts), np.ascontiguousarray(ref_faces, np.int32)
+        V = len(views)
+        vs = [_f32(v).reshape(-1, 3) for v, _ in views]
+        fs = [np.ascontiguousarray(f, np.int32).reshape(-1, 3) for _, f in views]
+        voff = np.zeros(V + 1, np.int64)
+        foff = np.zeros(V + 1, np.int64)
+        voff[1:] = np.cumsum([len(v) for v in vs])
+        foff[1:] = np.cumsum([len(f) for f in fs])
+        verts = np.ascontiguousarray(np.concatenate(vs) if V else np.zeros((0, 3), np.float32), np.float32)
+        faces = np.ascontiguousarray(np.concatenate(fs) if V else np.zeros((0, 3), np.int32), np.int32)
+        inter, uni = np.zeros(max(V, 1), np.int64), np.zeros(max(V, 1), np.int64)
+        grids = np.empty((V + 1, dim, dim, dim), np.uint8) if want_grids else None
+        ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+        check(self.lib.disn_iou_views(self._h, ptr(rv), len(rv), ptr(rf), len(rf), V, ptr(verts), ptr(voff), ptr(faces),
+                                      ptr(foff), dim, ptr(inter), ptr(uni), ptr(grids)))
+        inter, uni = inter[:V], uni[:V]
+        with np.errstate(invalid="ignore", divide="ignore"):
+            val = np.where(uni > 0, inter / np.maximum(uni, 1), np.nan)
+        return (val, inter, uni, grids) if want_grids else (val, inter, uni)
+
 
 def write_dist(path: str, res: int, bbox, values):
     """C-ABI .dist writer (test/create_sdf.py:292-303 layout)."""

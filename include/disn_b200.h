@@ -286,6 +286,18 @@ int disn_iou(disn_ctx* ctx, const float* verts1, int64_t nv1, const int32_t* fac
              int64_t nv2, const int32_t* faces2, int64_t nf2, int32_t dim, int64_t* intersection, int64_t* uni,
              uint8_t* occ1_out, uint8_t* occ2_out);
 
+/* One reference mesh against V meshes (the views of test/test_iou.py:165-206 iou_cat, one call per object): the reference
+ * is voxelised once, the V views in one launch, and the V intersection / union counts come back from one synchronise.
+ * View v has vertices [vert_offsets[v], vert_offsets[v+1]) of verts and faces [face_offsets[v], face_offsets[v+1]) of
+ * faces, whose ids are local to the view.  intersection[v] / uni[v] equal disn_iou(ref, view v) bit for bit (disn_iou is
+ * the V = 1 case).  occ_out: optional uint8[(V+1)*dim^3], the reference's grid then the views'.  Refused before anything
+ * is launched: null pointers, dim outside [2,512], V < 1, offsets that do not start at 0 or decrease, a mesh without
+ * faces, a face id outside its own mesh (the message names the view).  Scratch per call: (V+1) windows of
+ * (1.2 dim + 8)^3 bits and (V+1) grids of dim^3 bits. */
+int disn_iou_views(disn_ctx* ctx, const float* ref_verts, int64_t ref_nv, const int32_t* ref_faces, int64_t ref_nf,
+                   int32_t V, const float* verts, const int64_t* vert_offsets, const int32_t* faces,
+                   const int64_t* face_offsets, int32_t dim, int64_t* intersection, int64_t* uni, uint8_t* occ_out);
+
 /* Graph intermediates and the encoder/decoder split point of the reference (models/model_normalization.py:38-45,169-206,
  * 223-238); host pointers, synchronous, not the hot path:
  *   disn_eval_points_ex  = disn_eval_points + out_global / out_local [B,N,1] (end_points['pred_sdf_value_global'/'_local']);
