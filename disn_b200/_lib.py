@@ -12,6 +12,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libdisn_b200.so")
 
 DISN_DEVICE_PTR = 1
+DISN_OBJ_PARTS = 1
+DISN_ERR_OBJ_UNSUPPORTED = -5
 PREC_FP32 = 0
 PREC_BF16X3 = 1
 PREC_F16F8 = 2
@@ -91,6 +93,10 @@ EXPORTS = {
     "disn_eval_points_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p]),
     "disn_point_img_feat": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
+    "disn_obj_read": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                C.POINTER(C.c_int32)]),
+    "disn_obj_parts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]),
+    "disn_obj_read_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 # diagnostics (include/disn_b200_test.h), exported by libdisn_b200_test.so only
@@ -113,6 +119,7 @@ TEST_EXPORTS = {
     "disn_mesh_adaptive_phase_ms": (C.c_int, [C.c_void_p, C.c_void_p]),
     "disn_mesh_adaptive_bytes": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "disn_mesh_adaptive_edges": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    "disn_debug_obj_tokens": (C.c_int, [C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
 }
 
 _lib = None

@@ -18,7 +18,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
-from .create_sdf import read_obj, write_obj
+from .create_sdf import write_obj
 
 _ENGINE = None
 _LOCK = threading.Lock()
@@ -35,10 +35,9 @@ def _engine():
 def separate_single_mesh(src_mesh, tar_mesh):
     """clean_smallparts.py:27-36: write the mesh to tar_mesh + ".obj" and each component to tar_mesh + "_<i>.obj"
     (components in order of their smallest face; each with the vertices its faces reference, in their original order)."""
-    verts, faces = read_obj(src_mesh)
     with _LOCK:
         eng = _engine()
-        eng.load_mesh(verts, faces)
+        verts, faces = eng.read_obj(src_mesh, load=True)
         counts, labels = eng.clean_mesh(np.inf, -1.0, fetch=False, want_labels=True)   # keeps every component
     write_obj(tar_mesh + ".obj", verts, faces)
     for count in range(counts.n_components):
@@ -54,10 +53,9 @@ def separate_single_mesh(src_mesh, tar_mesh):
 def clean_single_mesh(src_mesh, tar_mesh, dist_thresh, num_thresh):
     """clean_smallparts.py:38-54: keep the components with more than max_count * num_thresh vertices whose centroid lies
     closer than dist_thresh to the origin, and write them to tar_mesh."""
-    verts, faces = read_obj(src_mesh)
     with _LOCK:
         eng = _engine()
-        eng.load_mesh(verts, faces)
+        eng.read_obj(src_mesh, load=True)
         verts, faces = eng.clean_mesh(dist_thresh, num_thresh)
     write_obj(tar_mesh, verts, faces)
     print("threshes:", str(dist_thresh), str(num_thresh), " clean: ", src_mesh, " create: ", tar_mesh)

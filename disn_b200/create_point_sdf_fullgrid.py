@@ -13,7 +13,6 @@ import os
 import numpy as np
 
 from .create_point_sdf_grid import _engine, check_insideout, write_obj_exact
-from .create_sdf import read_obj_parts
 
 
 def sample_sdf(cat_id, num_sample, bandwidth, iso_val, sdf_dict, sdf_res, reduce, engine=None, device_ptr=None):
@@ -55,11 +54,10 @@ def get_normalize_mesh(model_file, norm_sdf_file, cat_id, obj, sdf_sub_dir, engi
     """The largest part of the raw OBJ, transformed with the (c, m) of norm_sdf_file and written as
     <sdf_sub_dir>/pc_norm.obj -> (obj_file, centroid, m).  The part's vertices are the ones its faces reference, in their
     original order."""
-    verts, faces, pid, names = read_obj_parts(model_file)
-    centroid, m = get_param_from_h5(norm_sdf_file, cat_id, obj)
     eng, own = _engine(engine)
     try:
-        eng.load_mesh(verts, faces)
+        verts, faces, pid, names = eng.read_obj(model_file, parts=True, load=True)
+        centroid, m = get_param_from_h5(norm_sdf_file, cat_id, obj)
         keep = pid == largest_part(eng, pid, max(len(names), 1))
         used = np.zeros(len(verts), bool)
         used[faces[keep].reshape(-1)] = True

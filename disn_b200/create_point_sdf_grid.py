@@ -26,7 +26,7 @@ import os
 
 import numpy as np
 
-from .create_sdf import read_dist, read_obj, read_obj_parts
+from .create_sdf import read_dist
 from .engine import write_dist
 
 TOTAL_SURFACE_SAMPLES = 16384     # get_normalize_mesh's `total` (:170)
@@ -37,10 +37,10 @@ def create_one_sdf(sdfcommand, res, expand_rate, sdf_file, obj_file, indx, g=0.0
     """Signed distance field of the OBJ mesh on a (res+1)^3 grid over the cube around its AABB scaled by expand_rate,
     wall threshold g, written as a .dist (the box goes in the header).  Returns (grid, bbox)."""
     from .engine import Engine
-    verts, faces = read_obj(obj_file)
     eng = engine if engine is not None else Engine(device=0, precision="fp32")
     try:
-        grid, bbox = eng.mesh_sdf(int(res), expand_rate=float(expand_rate), sigma=float(g), verts=verts, faces=faces)
+        eng.read_obj(obj_file, load=True)
+        grid, bbox = eng.mesh_sdf(int(res), expand_rate=float(expand_rate), sigma=float(g))
     finally:
         if engine is None:
             eng.close()
@@ -145,12 +145,15 @@ def write_obj_exact(path, verts, faces):
 
 
 def get_normalize_mesh(model_file, norm_mesh_sub_dir, engine=None, mesh=None):
-    """get_normalize_mesh (:169-198) on the device: reads the OBJ (or takes mesh = read_obj_parts' tuple), leaves the
-    normalised mesh resident in the engine, writes <norm_mesh_sub_dir>/pc_norm.obj -> (obj_file, centroid, m)."""
+    """get_normalize_mesh (:169-198) on the device: reads the OBJ into the engine (or takes mesh = read_obj_parts' tuple),
+    leaves the normalised mesh resident in the engine, writes <norm_mesh_sub_dir>/pc_norm.obj -> (obj_file, centroid, m)."""
     eng, own = _engine(engine)
     try:
-        verts, faces, pid, names = mesh if mesh is not None else read_obj_parts(model_file)
-        eng.load_mesh(verts, faces)
+        if mesh is None:
+            verts, faces, pid, names = eng.read_obj(model_file, parts=True, load=True)
+        else:
+            verts, faces, pid, names = mesh
+            eng.load_mesh(verts, faces)
         centroid, m = normalize_resident(eng, pid, max(len(names), 1))
         obj_file = os.path.join(norm_mesh_sub_dir, "pc_norm.obj")
         write_obj_exact(obj_file, *eng.fetch_mesh())
@@ -242,11 +245,10 @@ def create_sdf_obj(sdfcommand, marching_cube_command, cat_mesh_dir, cat_norm_mes
         model_file = os.path.join(cat_mesh_dir, obj, "models", "model_normalized.obj")
     eng, own = _engine(engine)
     try:
-        verts, faces, pid, names = read_obj_parts(model_file)
         if normalize:
-            _, centroid, m = get_normalize_mesh(model_file, norm_mesh_sub_dir, eng, (verts, faces, pid, names))
+            _, centroid, m = get_normalize_mesh(model_file, norm_mesh_sub_dir, eng)
         else:
-            eng.load_mesh(verts, faces)
+            eng.read_obj(model_file, parts=True, load=True)
             centroid, m = np.zeros(3), 1.0
         R = res + 1
         ptr = eng.field_buffer(R)

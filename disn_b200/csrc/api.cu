@@ -24,6 +24,8 @@ disn_ctx::~disn_ctx() {
     if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : am_ev)
     if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : obj_ev)
+    if (e) cudaEventDestroy(e);
   if (own_stream && stream) cudaStreamDestroy(stream);
 }
 

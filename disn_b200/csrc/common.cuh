@@ -310,6 +310,20 @@ struct disn_ctx {
   cudaEvent_t am_ev[4] = {};
   int64_t am_nv = -1;
   const unsigned long long* am_edges_sorted = nullptr;
+  // OBJ reader (obj_read.cu): the file's bytes in pinned staging and on the device, the per-line arrays (line starts,
+  // record types, scanned counts, usemtl max-scan, select / scan scratch), the per-face and per-coordinate lists (face
+  // materials, host-converted coordinates), counters with their pinned mirror, the host side of the coordinate list, the
+  // per-face part ids and the part names of the last read (obj_none: the part of the faces before any usemtl), phase
+  // events and times (upload, line starts, classify, parse; host conversion and parts in [4])
+  disn::PinnedBuffer obj_host;
+  disn::DevBuffer obj_bytes, obj_arena, obj_lists, obj_small;
+  disn::PinnedBuffer obj_small_host, obj_list_host, obj_part_ids;
+  std::vector<std::string> obj_names;
+  std::vector<bool> obj_none;
+  bool obj_parts_ready = false;
+  int64_t obj_part_faces = 0, obj_host_tokens = 0, obj_overflows = 0;
+  cudaEvent_t obj_ev[5] = {};
+  float obj_phase_ms[5] = {};
   // nn_distance / cam scratch (persistent, grows)
   disn::DevBuffer nn_scratch;
   disn::DevBuffer dec_scratch;  // explicit-feature decoder staging (decoder.cu)
@@ -390,4 +404,7 @@ int adaptive_mesh_run(disn_ctx* c, const float* field, int image, const float* d
 int finish_mesh_call(disn_ctx* c, int rc, int64_t* n_verts, int64_t* n_faces);
 // bytes held by the buffers of adaptive_mesh_run
 size_t adaptive_mesh_bytes(const disn_ctx* c);
+// obj_read.cu: one OBJ coordinate token -> float32 as Python's float() and numpy's float64 -> float32 cast (-1 outside the
+// reader's grammar; *overflow set when a finite value becomes a float32 infinity)
+int obj_token_to_float(const char* s, int64_t len, float* out, bool* overflow);
 }  // namespace disn

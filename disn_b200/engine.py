@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
+import os
 from typing import NamedTuple
 
 import numpy as np
@@ -46,6 +47,7 @@ class Engine:
         self._mesh_faces = 0        # face count of the resident mesh (sizes clean_mesh's labels)
         self._mesh_verts = 0        # vertex count of the resident mesh (sizes fetch_mesh)
         self.last_clean = None
+        self.obj_fallbacks = 0      # files read_obj handed to the Python reader
 
     # -- lifetime -----------------------------------------------------------------------------
     def close(self):
@@ -321,6 +323,50 @@ class Engine:
         check(self.lib.disn_mesh_load(self._h, v.ctypes.data_as(C.c_void_p), len(v), f.ctypes.data_as(C.c_void_p), len(f)))
         self._mesh_faces = len(f)
         self._mesh_verts = len(v)
+
+    def read_obj(self, path, parts: bool = False, load: bool = False):
+        """create_sdf.read_obj(path), or read_obj_parts(path) with parts=True, parsed on the device (disn_obj_read): the
+        same arrays bit for bit, and the same names.  The mesh stays resident, as after load_mesh.  A file outside the
+        device reader's grammar (or one it finds invalid, or cannot open) is read by the Python reader instead, which
+        raises what it raises; `obj_fallbacks` counts those files, and load=True then uploads what it returned."""
+        nv, nf, npart = C.c_int64(0), C.c_int64(0), C.c_int32(0)
+        rc = self.lib.disn_obj_read(self._h, os.fsencode(path), _lib.DISN_OBJ_PARTS if parts else 0, C.byref(nv),
+                                    C.byref(nf), C.byref(npart))
+        self._mesh_verts, self._mesh_faces = nv.value, nf.value
+        if rc == _lib.DISN_ERR_OBJ_UNSUPPORTED:
+            from .create_sdf import read_obj, read_obj_parts
+            self.obj_fallbacks += 1
+            mesh = read_obj_parts(path) if parts else read_obj(path)
+            if load:
+                self.load_mesh(mesh[0], mesh[1])
+            return mesh
+        check(rc)
+        counts = np.zeros(2, np.int64)
+        check(self.lib.disn_obj_read_stats(self._h, counts.ctypes.data_as(C.c_void_p), None))
+        if counts[1]:       # a finite coordinate overflowed float32: numpy's own warning, as the cast in read_obj gives
+            np.array([np.finfo(np.float64).max]).astype(np.float32)
+        verts, faces = self.fetch_mesh()
+        if not parts:
+            return verts, faces
+        pid = np.empty(nf.value, np.int32)
+        off = np.empty(npart.value + 1, np.int64)
+        check(self.lib.disn_obj_parts(self._h, pid.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p), None, 0))
+        buf = C.create_string_buffer(max(int(off[-1]), 1))
+        check(self.lib.disn_obj_parts(self._h, None, None, buf, len(buf)))
+        names, end = [], int(off[-1])
+        for s in off[-2::-1]:           # a part's name ends where the next named part's begins (None has no bytes)
+            names.append(None if s < 0 else buf.raw[s:end].decode("ascii"))
+            end = end if s < 0 else int(s)
+        return verts, faces, pid, names[::-1]
+
+    def obj_read_stats(self):
+        """The last successful disn_obj_read: coordinates converted on the host, coordinates that overflowed float32, and
+        the milliseconds of its phases (device events: upload, lines, classify, parse; host clock: host)."""
+        counts = np.zeros(2, np.int64)
+        ms = (C.c_float * 5)()
+        check(self.lib.disn_obj_read_stats(self._h, counts.ctypes.data_as(C.c_void_p), ms))
+        return {"host_tokens": int(counts[0]), "overflows": int(counts[1]),
+                "phase_ms": dict(zip(("upload", "lines", "classify", "parse", "host"), list(ms)))}
 
     def fetch_mesh(self):
         """The resident mesh (last marching_cubes / load_mesh / clean_mesh / normalize_mesh) -> (verts, faces)."""

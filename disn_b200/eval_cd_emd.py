@@ -24,8 +24,7 @@ import random
 
 import numpy as np
 
-from .create_sdf import read_obj
-from .eval_common import listdir, read_lst, select_cats
+from .eval_common import listdir, read_lst, read_mesh, select_cats
 
 _ENGINE = None
 _DEVICE = 0
@@ -84,10 +83,10 @@ def cd_emd_cat(cat_id, cat_nm, pred_dir, gt_dir, test_lst_f, view_num=24, num_sa
         src_path = os.path.join(gt_dir, obj_id, "isosurf.obj")
         pred_path_lst = pred_dict[obj_id]
         verts_batch = np.zeros((view_num + 1, num_sample_points, 3), dtype=np.float32)
-        verts_batch[0, ...] = _sample(read_obj(src_path)[0], num_sample_points)
+        verts_batch[0, ...] = _sample(read_mesh(_engine(), src_path)[0], num_sample_points)
         pred_path_lst = random.sample(pred_path_lst, view_num)
         for i in range(len(pred_path_lst)):
-            verts = read_obj(pred_path_lst[i])[0]
+            verts = read_mesh(_engine(), pred_path_lst[i])[0]
             if verts.shape[0] > 0:
                 verts_batch[i + 1, ...] = _sample(verts, num_sample_points)
         if batch_size == view_num:
@@ -140,7 +139,7 @@ def sample_save_gt_pnt(cat_id, cat_nm, gt_dir_cat, test_lst_f, num_sample_points
     saved = []
     for obj_id in read_lst(test_lst_f):
         obj_path = os.path.join(gt_dir_cat, obj_id, "isosurf.obj")
-        verts_batch = _sample(read_obj(obj_path)[0], num_sample_points)
+        verts_batch = _sample(read_mesh(_engine(), obj_path)[0], num_sample_points)
         savefn = os.path.join(gt_dir_cat, obj_id, "pnt_{}.txt".format(num_sample_points))
         np.savetxt(savefn, verts_batch, delimiter=',')
         print("saved gt pnt of {} at {}".format(obj_id, savefn))
@@ -168,7 +167,7 @@ def sample_save_pred_pnt(cat_id, cat_nm, pred_dir, test_lst_f, view_num=24, num_
         verts_batch = np.zeros((view_num, num_sample_points, 3), dtype=np.float32)
         for i in range(len(pred_path_lst)):
             pred_mesh_fl = pred_path_lst[i]
-            verts = read_obj(pred_mesh_fl)[0]
+            verts = read_mesh(_engine(), pred_mesh_fl)[0]
             if verts.shape[0] > 0:
                 verts_batch[i, ...] = _sample(verts, num_sample_points)
             savedir = os.path.join(os.path.dirname(pred_dir), "pnt_{}_{}".format(num_sample_points, cat_id))

@@ -9,6 +9,8 @@ from __future__ import annotations
 
 import os
 
+from .create_sdf import read_obj
+
 CATS_ALL = {
     "watercraft": "04530566",
     "rifle": "04090263",
@@ -49,3 +51,10 @@ def read_lst(test_lst_f: str):
     """Object ids of <cat_id>_test.lst, one per line, with the line ends stripped as the reference does."""
     with open(test_lst_f, "r") as f:
         return [o.rstrip("\r\n") for o in f.readlines()]
+
+
+def read_mesh(engine, path):
+    """OBJ -> (verts, faces) through the engine's device reader (Engine.read_obj, bit for bit create_sdf.read_obj).  An
+    engine without a device reader -- a CPU stand-in for the evaluation methods -- reads with create_sdf.read_obj."""
+    reader = getattr(engine, "read_obj", None)
+    return reader(path) if reader is not None else read_obj(path)

@@ -19,8 +19,7 @@ import random
 
 import numpy as np
 
-from .create_sdf import read_obj
-from .eval_common import CATS_CLEAN_IOU, listdir, read_lst, select_cats
+from .eval_common import CATS_CLEAN_IOU, listdir, read_lst, read_mesh, select_cats
 
 _ENGINE = None
 _DEVICE = 0
@@ -35,7 +34,7 @@ def _engine():
 
 
 def _read_mesh(path):
-    verts, faces = read_obj(path)
+    verts, faces = read_mesh(_engine(), path)
     if len(faces) == 0:
         raise ValueError("%s: mesh has no faces, its IoU is undefined" % path)
     return verts, faces

@@ -25,6 +25,9 @@
  *   disn_mesh_sdf                   <-> os.system("computeDistanceField <obj> res res res -s -e <e> -o X.dist -m 1 [-g s]")
  *                                       (preprocessing/create_point_sdf_grid.py:200-210)
  *   disn_mesh_part_areas / disn_mesh_normalize <-> get_normalize_mesh (preprocessing/create_point_sdf_grid.py:169-198)
+ *   disn_obj_read / disn_obj_parts  <-> pymesh.load_mesh (test/test_cd_emd.py:180-250, test/test_iou.py:210,220,
+ *                                       postprocessing/clean_smallparts.py:28,39) and trimesh.load_mesh(process=False)
+ *                                       (preprocessing/create_point_sdf_grid.py:172, create_point_sdf_fullgrid.py:166)
  *   disn_field / disn_sdf_band_count / disn_sdf_band_gather <-> the field between create_one_sdf, create_one_cube_obj
  *                                       and sample_sdf (:74-113, :200-252); disn_sdf_strided <-> the strided sample_sdf
  *                                       of create_point_sdf_fullgrid.py:70-96
@@ -49,6 +52,12 @@ typedef struct disn_ctx disn_ctx;
 
 enum {
   DISN_DEVICE_PTR = 1,   /* data pointers are device pointers; call is async on the ctx stream */
+};
+
+enum {
+  DISN_OBJ_PARTS = 1,               /* disn_obj_read: also record per-face material parts for disn_obj_parts */
+  DISN_ERR_OBJ_UNSUPPORTED = -5,    /* disn_obj_read: the file cannot be opened, lies outside the reader's grammar or is
+                                       invalid; disn_last_error() names the path, the line and the reason */
 };
 
 /* arithmetic used by the fused point kernel */
@@ -186,6 +195,27 @@ int disn_fetch(disn_ctx* ctx, const void* dev, void* host, int64_t bytes);
 int disn_mesh_load(disn_ctx* ctx, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces);
 int disn_mesh_clean(disn_ctx* ctx, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
                     int64_t* n_kept, int64_t* n_verts, int64_t* n_faces);
+
+/* OBJ file -> the resident mesh, parsed on the device (create_sdf.read_obj / read_obj_parts; pymesh.load_mesh /
+ * trimesh.load_mesh(process=False) in the reference).  On success the context is in the state disn_mesh_load of
+ * read_obj's arrays leaves: verts [V,3] float32 (each coordinate float64-rounded, then float32-rounded), faces [F,3] int32
+ * 0-based.  The grammar: ASCII; lines end at \n, \r\n or a lone \r; tokens split on space, \t, \v, \f, \x1c-\x1f; `v`
+ * records take tokens 1-3 as [+-]?(digits[.digits?]|.digits)([eE][+-]?digits)? or inf / infinity / nan; `f` records have
+ * exactly three corners whose text before the first '/' is [+-]?digits (at most 18) in [1, V], V counted over the whole
+ * file; other records are ignored.  Anything else returns DISN_ERR_OBJ_UNSUPPORTED and leaves the resident mesh empty,
+ * as does every other failure (CUDA and allocation errors keep their ordinary codes).  *n_verts / *n_faces / *n_parts
+ * (each may be NULL) receive the resident counts and the number of parts.
+ * disn_obj_parts (after a read with DISN_OBJ_PARTS): part_ids [n_faces] int32 = the part of each face, parts numbered in
+ * order of their first face; a face's part is the material name of the last `usemtl` line before it (its second token,
+ * or "" when it has none).  Part p's name is names[name_offsets[p] .. the next part's non-negative offset, or
+ * name_offsets[n_parts]); the part of faces before any usemtl has offset -1.  Any of part_ids / name_offsets / names may
+ * be NULL (name_offsets[n_parts] is the bytes names needs).
+ * disn_obj_read_stats: counts[2] = coordinates of the last read converted on the host (those outside the device's exact
+ * rule), coordinates whose finite float64 value overflowed float32; phase_ms[5] = upload, line starts, classification,
+ * parse (device events) and host conversion + parts (host clock) of the last successful read. */
+int disn_obj_read(disn_ctx* ctx, const char* path, uint32_t flags, int64_t* n_verts, int64_t* n_faces, int32_t* n_parts);
+int disn_obj_parts(disn_ctx* ctx, int32_t* part_ids, int64_t* name_offsets, char* names, int64_t names_capacity);
+int disn_obj_read_stats(disn_ctx* ctx, int64_t* counts, float* phase_ms);
 
 /* Signed distance field of the resident mesh (disn_mesh_load / disn_mc_run / disn_mesh_clean), the reference's
  * computeDistanceField -s (preprocessing/create_point_sdf_grid.py:200-210): R = res+1 points per axis over bbox

@@ -56,6 +56,11 @@ int disn_mesh_adaptive_phase_ms(disn_ctx* ctx, float* ms);
 int disn_mesh_adaptive_bytes(disn_ctx* ctx, int64_t* bytes);
 int disn_mesh_adaptive_edges(disn_ctx* ctx, int64_t first, int64_t n, int64_t* out);
 
+/* Diagnostic: the OBJ reader's host coordinate converter (Python's float() then numpy's float64 -> float32 cast) on n
+ * tokens text[offsets[i] .. offsets[i] + lengths[i]) -> out[n]; a token outside the reader's grammar is an error naming
+ * it.  Needs no device. */
+int disn_debug_obj_tokens(const char* text, const int64_t* offsets, const int32_t* lengths, int64_t n, float* out);
+
 #ifdef __cplusplus
 }
 #endif

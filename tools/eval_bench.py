@@ -6,8 +6,9 @@ Engine.iou_views against one Engine.iou call per view.
 The object: the ground truth is the marching-cubes mesh of the 257^3 grid of the synthetic He-scaled network on the demo
 image and camera at the median of its field; the 24 views are the meshes of its 65^3 grid at 24 isovalues around that
 median.  The meshes are written as OBJ files and read back as the drivers read them.  Per driver and object, host
-wall-clock (time.perf_counter; every GPU call ends in a synchronise) of: OBJ / point-file parsing, sampling, and the
-GPU metric calls, median of --reps.  iou_views and 24 x iou first check that their counts are equal.  Prints one JSON
+wall-clock (time.perf_counter; every GPU call ends in a synchronise) of: OBJ parsing as the drivers do it
+(Engine.read_obj; the Python reader's time is reported beside it as python_parse_ms) / point-file parsing, sampling, and
+the GPU metric calls, median of --reps.  iou_views and 24 x iou first check that their counts are equal.  Prints one JSON
 line with the GPU name and power limit read in the same run; also writes it to DIR/eval_bench.json.
 """
 import argparse
@@ -76,7 +77,10 @@ def main():
         for p, (v, f) in zip(paths, views):
             write_obj(p, v, f)
         read_all = lambda: [read_obj(gt_path)] + [read_obj(p) for p in paths]
-        parse_ms, meshes = timed(read_all, args.reps)
+        python_parse_ms, py_meshes = timed(read_all, args.reps)
+        parse_ms, meshes = timed(lambda: [eng.read_obj(gt_path)] + [eng.read_obj(p) for p in paths], args.reps)
+        assert eng.obj_fallbacks == 0 and all(a.tobytes() == b.tobytes() for m, n in zip(meshes, py_meshes)
+                                              for a, b in zip(m, n)), "Engine.read_obj != read_obj"
 
         def sample():
             np.random.seed(0)
@@ -107,9 +111,11 @@ def main():
         pair_ms, pr = timed(pairs, args.reps)
         assert [(int(a), int(b)) for a, b in zip(inter, uni)] == [tuple(p) for p in pr], "iou_views != 24 x iou"
         rows["iou"] = dict(parse_ms=parse_ms, sample_ms=0.0, gpu_ms=iv_ms, gpu_ms_24_separate_iou=pair_ms)
-    for r in rows.values():
+    for k, r in rows.items():
         r["total_ms"] = r["parse_ms"] + r["sample_ms"] + r["gpu_ms"]
         r["parse_share"] = r["parse_ms"] / r["total_ms"]
+        if k != "f_score":
+            r["python_parse_ms"] = python_parse_ms
     eng.close()
     out = {"gpu": gpu_info(), "reps": args.reps, "views": V, "num_sample_points": N, "dim": DIM,
            "gt_mesh": {"grid": "257^3", "verts": int(len(gt[0])), "faces": int(len(gt[1]))},
