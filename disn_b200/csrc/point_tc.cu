@@ -183,6 +183,7 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
     const int64_t tile = (int64_t)blockIdx.x + (int64_t)it * gridDim.x;
     const int b = (int)(tile / tiles_per_img);
     const int64_t n0 = (tile % tiles_per_img) * PTS;
+#pragma unroll(kMode == MODE_F16F8 ? 2 : 1)
     for (int sx = 0; sx < 2; ++sx) {
       // ---- fold1/conv1 (3 -> 64, fp32 FMA) into K slice 0: thread -> point tid / 4, features 16 (tid % 4) + [0, 16)
       named_bar_sync(1, NCONS);                  // the previous layer's MMAs are done with the activation buffer
@@ -319,10 +320,12 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
 #pragma unroll
               for (int e2 = 0; e2 < 2; ++e2) {
                 float v2[2] = {bias[0], bias[1]};
-                // layer 2 shares its code between the streams: the tap loads stay unconditional (every address is valid)
-                // so that the compiler can issue them ahead across j; a branch around them per j serialised their L2
-                // round trips.  Only the local stream adds the result.
-                if (layer == 2) {
+                // only the local stream adds the gather.  MODE_F16F8 compiles each stream's epilogues apart (the stream
+                // loop is unrolled), so `gather` is a constant there and the global stream issues no tap loads.
+                // MODE_BF16X3 shares layer 2's code between the streams (unrolled, it spills inside its epilogues):
+                // its tap loads stay unconditional (every address is valid) so that the compiler can issue them ahead
+                // across j; a branch around them per j serialised their L2 round trips.
+                if (layer == 2 && (gather || kMode == MODE_BF16X3)) {
                   float2 a = make_float2(0.f, 0.f);
 #pragma unroll
                   for (int k = 0; k < 4; ++k) {
