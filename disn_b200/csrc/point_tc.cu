@@ -38,6 +38,7 @@
 #include <cuda_fp8.h>
 
 #include "common.cuh"
+#include "point_tc_layout.cuh"
 #include "tc_common.cuh"
 
 namespace disn {
@@ -49,9 +50,9 @@ constexpr int NSLOT = 3;              // weight ring slots
 constexpr int W_TILE = 16384;         // 128 rows x 64 k x 2 B (SW128)
 constexpr int W8_TILE = 8192;         // 128 rows x 64 k x 1 B (SW64)
 constexpr int HS_BYTES = 2 * W_TILE;  // half-stage: [W_hi | W_lo] or [fp16 W | e5m2 W | e5m2 residual of W]
-constexpr int X_TILE = 8192;          // 64 rows x 64 k x 2 B (SW128)
-constexpr int X8_TILE = 4096;         // 64 rows x 64 k x 1 B (SW64)
-constexpr int X_SLICE = 2 * X_TILE;   // one 64-wide K slice: [hi | lo] or [fp16 | e5m2 residual | e5m2 copy]
+using ptc::X_TILE;                     // 64 rows x 64 k x 2 B (SW128)
+using ptc::X8_TILE;                    // 64 rows x 64 k x 1 B (SW64)
+using ptc::X_SLICE;                    // one 64-wide K slice: [hi | lo] or [fp16 | e5m2 residual | e5m2 copy]
 constexpr int STAGES_PER_STREAM = 33; // 1 + 8 + 16 + 8 (K slice, 256-wide N block) stages
 constexpr int HS_PER_TILE = 2 * 2 * STAGES_PER_STREAM;
 // correction products DISN_PREC_F16F8 keeps in each tensor layer l = 0..3 (fold1/conv2, fold1/conv3, fold2/conv1,
@@ -105,29 +106,31 @@ __device__ __forceinline__ void taps_of(const PointJob& job, int b, int64_t n, i
   }
 }
 
-// write activations (a, b) of features (k, k+1) of point `row` into K slice `xs` in the operand format of kMode.
-// MODE_F16F8 also folds the fp16 values into `amax` (all values are post-ReLU, i.e. >= 0): an activation above fp16's
-// 65504 becomes +inf there, which the kernel reports through PointJob::status instead of producing a silent inf.
+static_assert(ptc::store_offset_mismatches() == 0, "epilogue / prologue store offsets disagree with the swizzled layout");
+
+// write activations (a, b) of two adjacent features of one point into the activation buffer `x` in the operand format
+// of kMode: the 2-byte pair at byte offset o16 (ptc::epi_off16 / pro_off16), MODE_F16F8's e5m2 pairs at o8
+// (ptc::epi_off8 / pro_off8).  MODE_F16F8 also folds the fp16 values into `amax` (all values are post-ReLU, i.e. >= 0):
+// an activation above fp16's 65504 becomes +inf there, which the kernel reports through PointJob::status instead of
+// producing a silent inf.
 template <int kMode>
-__device__ __forceinline__ void store_pair(uint8_t* xs, int row, int k, float a, float b, float sc_lo, float sc_hi,
-                                           __half2& amax) {
-  const uint32_t off = tc::sw128_offset((uint32_t)row, (uint32_t)(k >> 3)) + (uint32_t)(k & 7) * 2u;
+__device__ __forceinline__ void store_pair(uint8_t* x, uint32_t o16, uint32_t o8, float a, float b, float sc_lo,
+                                           float sc_hi, __half2& amax) {
   if constexpr (kMode == MODE_BF16X3) {
     uint32_t hi, lo;
     tc::split_bf16x2(a, b, hi, lo);
-    *reinterpret_cast<uint32_t*>(xs + off) = hi;
-    *reinterpret_cast<uint32_t*>(xs + X_TILE + off) = lo;
+    *reinterpret_cast<uint32_t*>(x + o16) = hi;
+    *reinterpret_cast<uint32_t*>(x + o16 + X_TILE) = lo;
   } else {
     const __half2 hh = __floats2half2_rn(a, b);
     amax = __hmax2(amax, hh);
-    *reinterpret_cast<__half2*>(xs + off) = hh;
+    *reinterpret_cast<__half2*>(x + o16) = hh;
     const float ra = a - __low2float(hh), rb = b - __high2float(hh);      // fp16 rounding residual (first correction)
     const __nv_fp8x2_storage_t l = __nv_cvt_float2_to_fp8x2(make_float2(ra * sc_lo, rb * sc_lo), __NV_SATFINITE, __NV_E5M2);
     const __half2 hs = __hmul2(hh, __float2half2_rn(sc_hi));   // power-of-two scale: exact up to fp16 underflow
     const __nv_fp8x2_storage_t g = __nv_cvt_halfraw2_to_fp8x2(*reinterpret_cast<const __half2_raw*>(&hs), __NV_SATFINITE, __NV_E5M2);
-    const uint32_t o8 = tc::sw64_offset((uint32_t)row, (uint32_t)(k >> 4)) + (uint32_t)(k & 15);
-    *reinterpret_cast<__nv_fp8x2_storage_t*>(xs + X_TILE + o8) = l;
-    *reinterpret_cast<__nv_fp8x2_storage_t*>(xs + X_TILE + X8_TILE + o8) = g;
+    *reinterpret_cast<__nv_fp8x2_storage_t*>(x + o8) = l;
+    *reinterpret_cast<__nv_fp8x2_storage_t*>(x + o8 + X8_TILE) = g;
   }
 }
 
@@ -199,12 +202,16 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
           o[0] = u; o[1] = v;
         }
         const StreamWeights& sw = sx ? job.l : job.g;
+        const float* b1p = sw.b1 + f0;
+        const float* w1p = sw.w1 + f0;
+        const uint32_t o16 = ptc::pro_base16((uint32_t)p, (uint32_t)(tid & 3));
+        const uint32_t o8 = ptc::pro_base8((uint32_t)p, (uint32_t)(tid & 3));
 #pragma unroll
         for (int j = 0; j < 16; j += 2) {
-          const float2 b1 = __ldg(reinterpret_cast<const float2*>(sw.b1 + f0 + j));
-          const float2 wx = __ldg(reinterpret_cast<const float2*>(sw.w1 + f0 + j));
-          const float2 wy = __ldg(reinterpret_cast<const float2*>(sw.w1 + 64 + f0 + j));
-          const float2 wz = __ldg(reinterpret_cast<const float2*>(sw.w1 + 128 + f0 + j));
+          const float2 b1 = __ldg(reinterpret_cast<const float2*>(b1p + j));
+          const float2 wx = __ldg(reinterpret_cast<const float2*>(w1p + j));
+          const float2 wy = __ldg(reinterpret_cast<const float2*>(w1p + 64 + j));
+          const float2 wz = __ldg(reinterpret_cast<const float2*>(w1p + 128 + j));
           float v2[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
@@ -214,7 +221,8 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
             a = fmaf(zr, e ? wz.y : wz.x, a);
             v2[e] = fmaxf(a, 0.f);
           }
-          store_pair<kMode>(s.x[0], p, f0 + j, v2[0], v2[1], job.act_scale[sx][0][0], job.act_scale[sx][0][1], amax);
+          store_pair<kMode>(s.x[0], ptc::pro_off16(o16, j), ptc::pro_off8(o8, j), v2[0], v2[1], job.act_scale[sx][0][0],
+                            job.act_scale[sx][0][1], amax);
         }
       }
       tc::fence_proxy_async_smem();
@@ -299,23 +307,31 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
 #pragma unroll
             for (int k = 0; k < 8; ++k) { off[k >> 2][k & 3] = -1; wg[k >> 2][k & 3] = 0.f; }
           }
-          const float* pm = job.pfeat ? job.pfeat : job.pmap + (int64_t)b * job.img_h * job.img_w * kHidden;
           const StreamWeights& sw = sx ? job.l : job.g;
           const float* bias_v = layer == 0 ? sw.b2 : (layer == 1 ? sw.b3 : (sx == 0 ? job.gbias + (int64_t)b * kHidden : sw.b4));
           const float sc_lo = job.act_scale[sx][layer + 1][0], sc_hi = job.act_scale[sx][layer + 1][1];
-          // MODE_F16F8: the thread's row and column bases, made opaque here so that the epilogue's ~100 store offsets are
-          // derived from them in place: the compiler would otherwise hoist them out of the tile loop and keep them live
-          // across the MMA loops next to the main and side accumulators, where they spill.  MODE_BF16X3 has the
-          // registers to keep them, and recomputing them costs it time.
+          // Every address of the epilogue is a per-thread base plus an immediate: the parameter and tap pointers point
+          // at this thread's first column (feature 128h + cq), the store bases hold its row's swizzle pattern
+          // (point_tc_layout.cuh), and N block, column group and row half are offsets from them.
+          // MODE_F16F8: the thread's row and column are made opaque here so that the bases are formed in place: the
+          // compiler would otherwise hoist them out of the tile loop and keep them live across the MMA loops next to
+          // the main and side accumulators, where they spill.  MODE_BF16X3 has the registers to keep them.
           int row = r0, cbase = h * 128 + cq;
           if constexpr (kMode == MODE_F16F8) asm volatile("" : "+r"(row), "+r"(cbase));
+          const uint32_t base16 = ptc::epi_base16((uint32_t)cbase >> 7, (uint32_t)row, (uint32_t)cbase & 127u);
+          const uint32_t base8 = ptc::epi_base8((uint32_t)cbase >> 7, (uint32_t)row, (uint32_t)cbase & 127u);
+          const float* bp = bias_v + cbase;
+          // the four taps of rows r0 and r0 + 8 (an outside tap reads the first row of the map with weight 0)
+          const float* pm = (job.pfeat ? job.pfeat : job.pmap + (int64_t)b * job.img_h * job.img_w * kHidden) + cbase;
+          const float* tp[2][4];
+#pragma unroll
+          for (int k = 0; k < 8; ++k) tp[k >> 2][k & 3] = pm + max(off[k >> 2][k & 3], 0);
 #pragma unroll
           for (int nb = 0; nb < 2; ++nb) {
             if (nb >= nnb) continue;
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
-              const int col = nb * 256 + cbase + 8 * j;
-              const float2 bb = __ldg(reinterpret_cast<const float2*>(bias_v + col));
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(bp + nb * 256 + 8 * j));
               const float bias[2] = {bb.x, bb.y};
 #pragma unroll
               for (int e2 = 0; e2 < 2; ++e2) {
@@ -329,8 +345,7 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
                   float2 a = make_float2(0.f, 0.f);
 #pragma unroll
                   for (int k = 0; k < 4; ++k) {
-                    const int o = off[e2][k];
-                    const float2 m = __ldg(reinterpret_cast<const float2*>(pm + (o >= 0 ? o : 0) + col));
+                    const float2 m = __ldg(reinterpret_cast<const float2*>(tp[e2][k] + nb * 256 + 8 * j));
                     a.x = fmaf(wg[e2][k], m.x, a.x);
                     a.y = fmaf(wg[e2][k], m.y, a.y);
                   }
@@ -341,7 +356,8 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
                 }
                 const float va = fmaxf(acc[nb][4 * j + 2 * e2] + v2[0], 0.f);
                 const float vb = fmaxf(acc[nb][4 * j + 2 * e2 + 1] + v2[1], 0.f);
-                store_pair<kMode>(s.x[col >> 6], row + 8 * e2, col & 63, va, vb, sc_lo, sc_hi, amax);
+                store_pair<kMode>(s.x[0], ptc::epi_off16(base16, nb, j, e2), ptc::epi_off8(base8, nb, j, e2), va, vb,
+                                  sc_lo, sc_hi, amax);
               }
             }
           }
@@ -351,11 +367,12 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
           // ---- fold2/conv2 output (256) -> ReLU -> fold2/conv5 dot product
           float pr[2] = {0.f, 0.f};
           const StreamWeights& sw = sx ? job.l : job.g;
+          const float* b5p = sw.b5 + (h * 128 + cq);
+          const float* w6p = sw.w6 + (h * 128 + cq);
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            const int col = h * 128 + 8 * j + cq;
-            const float2 b5 = __ldg(reinterpret_cast<const float2*>(sw.b5 + col));
-            const float2 w6 = __ldg(reinterpret_cast<const float2*>(sw.w6 + col));
+            const float2 b5 = __ldg(reinterpret_cast<const float2*>(b5p + 8 * j));
+            const float2 w6 = __ldg(reinterpret_cast<const float2*>(w6p + 8 * j));
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
               const float a = fmaxf(acc[0][4 * j + e] + ((e & 1) ? b5.y : b5.x), 0.f);
