@@ -97,6 +97,8 @@ EXPORTS = {
                                 C.POINTER(C.c_int32)]),
     "disn_obj_parts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]),
     "disn_obj_read_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "disn_sdf_metrics": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_float,
+                                   C.c_float, C.c_float, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 # diagnostics (include/disn_b200_test.h), exported by libdisn_b200_test.so only

@@ -11,7 +11,7 @@ LIB = os.path.join(HERE, "libdisn_b200.so")
 TEST_LIB = os.path.join(HERE, "libdisn_b200_test.so")
 SOURCES = ["api.cu", "encoder.cu", "point_fp32.cu", "point_tc.cu", "mc.cu", "chamfer.cu", "conv_tc.cu", "cam.cu", "iou.cu",
            "decoder.cu", "emd.cu", "mesh_clean.cu", "mesh_sdf.cu", "mesh_normalize.cu", "sdf_sample.cu", "adaptive.cu",
-           "adaptive_mesh.cu", "obj_read.cu"]
+           "adaptive_mesh.cu", "obj_read.cu", "sdf_acc.cu"]
 # diagnostics: selftests / probes, plus encoder.cu rebuilt with its debug GEMM harness -> libdisn_b200_test.so
 DIAG_SOURCES = ["tc_selftest.cu", "tc_probe.cu", "adaptive_diag.cu", "tc_diag.cu", "obj_diag.cu"]
 # voxel classification (iou.cu), the small-part keep rule (mesh_clean.cu) and the distances and edge crossings of the

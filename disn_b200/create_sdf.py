@@ -1,8 +1,9 @@
 """Drop-in mirror of the reference's inference driver ``test/create_sdf.py`` (and ``demo/demo.py``) for the
 SDF hot path: same module-level constants, same function names and argument meaning
 (``create``, ``test_one_epoch``, ``to_binary``, ``create_obj``, ``create_one_cube_obj``), running on the
-DISN library.  Dataset loading (``TEST_DATASET``: h5 files on disk) is out of scope: ``create`` takes an
-iterable of ``batch_data`` dicts in the loader's layout (data/data_sdf_h5_queue.py:291-303).
+DISN library.  ``create`` takes an iterable of ``batch_data`` dicts in the loader's layout
+(data/data_sdf_h5_queue.py:291-303); ``python -m disn_b200.create_sdf`` feeds it from the test-set loader
+(disn_b200/data_sdf_h5_queue.py) over the view files of create_img_h5, as the reference script does.
 
     import disn_b200.create_sdf as cs
     cs.configure(FLAGS)                       # the reference does this at import time from argparse
@@ -307,3 +308,50 @@ def create_one_cube_obj(marching_cube_command, i, sdf_file, cube_obj_file):
             eng.close()
     write_obj(cube_obj_file, verts, faces)
     return cube_obj_file
+
+
+def main(argv=None, weights=None):
+    """`python -m disn_b200.create_sdf`: test/create_sdf.py as a script -- the test lists (test/create_sdf.py:106-149:
+    random.sample(range(24), view_num) views per object), the test-set loader without shuffling, and create().  weights
+    (TF variable name -> array) replaces the checkpoint of --log_dir."""
+    import argparse
+    import random
+    from . import data_sdf_h5_queue
+    from .test_sdf_acc import CATS, build_listinfo, checkpoint_prefix
+    ap = argparse.ArgumentParser()
+    d = default_flags()
+    for k in ("gpu", "log_dir", "category", "precision"):
+        ap.add_argument("--" + k, default=d.__dict__[k])
+    for k in ("max_epoch", "img_h", "img_w", "batch_size", "num_classes", "num_points", "sdf_res", "cat_limit",
+              "num_sample_points", "view_num"):
+        ap.add_argument("--" + k, type=int, default=dict(max_epoch=1, cat_limit=168000).get(k, d.__dict__.get(k)))
+    ap.add_argument("--iso", type=float, default=0.0)
+    for k in ("alpha", "rot", "tanh", "multi_view", "threedcnn", "img_feat_onestream", "binary", "create_obj", "store",
+              "cam_est", "augcolorfore", "augcolorback", "backcolorwhite", "adaptive", "clean_smallparts", "keep_dist"):
+        ap.add_argument("--" + k, action="store_true")
+    ap.add_argument("--img_feat_twostream", action="store_true", default=True)
+    ap.add_argument("--test_lst_dir", required=True, help="<cat_id>_test.lst")
+    ap.add_argument("--view_dir", required=True, help="view files of create_img_h5: <view_dir>/<cat>/<obj>/%%02d.npz")
+    ap.add_argument("--sdf_dir", required=True, help="<sdf_dir>/<cat>/<obj>/ori_sample.npz")
+    flags = ap.parse_args(argv)
+    print(flags)
+    data_sdf_h5_queue.check_flags(flags)
+    listinfo, cats_limit = build_listinfo(flags, CATS, view_lists=lambda: random.sample(range(24), flags.view_num))
+    dataset = data_sdf_h5_queue.Pt_sdf_img(flags, listinfo=listinfo, cats_limit=cats_limit, shuffle=False,
+                                           info={"rendered_dir": flags.view_dir, "sdf_dir": flags.sdf_dir})
+    configure(flags)
+    if weights is None:
+        from .tf_checkpoint import load_checkpoint
+        prefix = checkpoint_prefix(flags.log_dir)
+        weights = None if prefix is None else load_checkpoint(prefix, prefixes=("vgg_16/", "sdfprediction"))
+    num_batches = int(len(dataset) / BATCH_SIZE)
+    dataset.start()
+    try:
+        return create(weights, (dataset.fetch() for _ in range(num_batches)))
+    finally:
+        dataset.shutdown()
+        LOG_FOUT.close()
+
+
+if __name__ == "__main__":
+    main()

@@ -87,8 +87,10 @@ void disn_destroy(disn_ctx* c) {
   delete c;
 }
 
+}  // extern "C"
+
 // Call after a synchronisation of c->stream: turns failure bits the kernels raised into a loud error.
-static int check_status(disn_ctx* c) {
+int disn::check_status(disn_ctx* c) {
   int* h = c->h_status.as<int>();
   const int st = *h;
   if (st == 0) return 0;
@@ -106,6 +108,8 @@ static int check_status(disn_ctx* c) {
   set_error("kernel reported status " + std::to_string(st));
   return -4;
 }
+
+extern "C" {
 
 int disn_set_stream(disn_ctx* c, void* cuda_stream) {
   DISN_REQUIRE(c, "null ctx");

@@ -327,6 +327,7 @@ struct disn_ctx {
   // nn_distance / cam scratch (persistent, grows)
   disn::DevBuffer nn_scratch;
   disn::DevBuffer dec_scratch;  // explicit-feature decoder staging (decoder.cu)
+  disn::DevBuffer d_gt, d_acc;  // disn_sdf_metrics: host-call staging of the samples' values and the per-image sums
 };
 
 namespace disn {
@@ -338,6 +339,7 @@ void encoder_graph_reset(disn_ctx* c);
 // api.cu
 int run_point_job(disn_ctx* c, PointJob& job);    // fills weights / encoder products / status and launches per cfg.precision
 int ensure_point_scratch(disn_ctx* c, int64_t pts);
+int check_status(disn_ctx* c);    // after a synchronisation: the kernels' status bits as an error (and clears them)
 // encoder.cu helpers reused by the explicit-feature decoder
 int encoder_gemv(disn_ctx* c, const float* x, const float* W, const float* bias, float* out, int B, int K, int N, int relu);
 int encoder_gemm_plain(disn_ctx* c, const std::string& wname, const float* A, const float* Bm, const float* bias, float* C,

@@ -171,6 +171,34 @@ class Engine:
                                         C.c_void_p(trans_mat_ptr), B, N, C.c_void_p(out_ptr),
                                         C.c_void_p(uv_ptr or 0), DISN_DEVICE_PTR))
 
+    def sdf_metrics(self, pts, trans_mat, sdf_val, iso_offset: float = 0.003, sdf_weight: float = 10.0,
+                    mask_weight: float = 4.0, want_pred: bool = False):
+        """Per-image metrics of test/test_sdf_acc.py at ground-truth samples (disn_sdf_metrics): pts [B,N,3], trans_mat
+        [B,4,3], sdf_val [B,N] or [B,N,1] of the encoded batch -> (count int64 [B], wsum float64 [B], rsum float64 [B]),
+        and pred_sdf [B,N,1] (bitwise eval_points's) with want_pred.  batch_losses turns them into the batch values."""
+        p, t = _f32(pts), _f32(trans_mat)
+        if p.ndim != 3 or p.shape[2] != 3:
+            raise ValueError("pts must be [B,N,3]")
+        B, N, _ = p.shape
+        g = _f32(sdf_val)
+        if g.size != B * N:
+            raise ValueError("sdf_val must hold B*N values")
+        cnt, ws, rs = np.empty(B, np.int64), np.empty(B, np.float64), np.empty(B, np.float64)
+        pred = np.empty((B, N, 1), np.float32) if want_pred else None
+        ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+        check(self.lib.disn_sdf_metrics(self._h, ptr(p), ptr(t), ptr(g), B, N, float(iso_offset), float(sdf_weight),
+                                        float(mask_weight), 0, ptr(pred), ptr(cnt), ptr(ws), ptr(rs)))
+        return (cnt, ws, rs, pred) if want_pred else (cnt, ws, rs)
+
+    def sdf_metrics_device(self, pts_ptr: int, trans_mat_ptr: int, sdf_val_ptr: int, B: int, N: int, count_ptr: int,
+                           wsum_ptr: int, rsum_ptr: int, pred_ptr: int = 0, iso_offset: float = 0.003,
+                           sdf_weight: float = 10.0, mask_weight: float = 4.0):
+        """Device-pointer, asynchronous variant: int64 counts and float64 sums [B] at the given device addresses."""
+        check(self.lib.disn_sdf_metrics(self._h, C.c_void_p(pts_ptr), C.c_void_p(trans_mat_ptr), C.c_void_p(sdf_val_ptr),
+                                        B, N, float(iso_offset), float(sdf_weight), float(mask_weight), DISN_DEVICE_PTR,
+                                        C.c_void_p(pred_ptr or 0), C.c_void_p(count_ptr), C.c_void_p(wsum_ptr),
+                                        C.c_void_p(rsum_ptr)))
+
     def eval_grid(self, sdf_params, trans_mat, sdf_res: int, z0: int = 0, z1: int | None = None, out=None):
         """Dense grid slab -> [B, z1-z0, R, R] float32 = pred/sdf_weight (reference `result`, reshaped)."""
         sp = np.ascontiguousarray(sdf_params, dtype=np.float64).reshape(-1, 6)
@@ -653,6 +681,16 @@ class Engine:
         with np.errstate(invalid="ignore", divide="ignore"):
             val = np.where(uni > 0, inter / np.maximum(uni, 1), np.nan)
         return (val, inter, uni, grids) if want_grids else (val, inter, uni)
+
+
+def batch_losses(count, wsum, rsum, n_values: int):
+    """The batch values of test_sdf_acc from per-image sdf_metrics results summed over n_values = B*N samples:
+    (accuracy, sdf_loss_realvalue, sdf_loss) as float32.  accuracy equals np.mean of the 0/1 float32 agreements bit for
+    bit (both operands are exact below 2^24)."""
+    acc = np.float32(int(np.sum(count))) / np.float32(n_values)
+    real = np.float32(float(np.sum(rsum)) / n_values)
+    loss = np.float32(float(np.sum(wsum)) / n_values) * np.float32(1000)
+    return acc, real, loss
 
 
 def write_dist(path: str, res: int, bbox, values):

@@ -32,10 +32,12 @@ def intrinsics() -> np.ndarray:
     return np.array([[F_PIX, 0.0, C_PIX], [0.0, F_PIX, C_PIX], [0.0, 0.0, 1.0]], dtype=np.float64)
 
 
-def blender_extrinsics(az_deg: float, el_deg: float, distance_ratio: float) -> np.ndarray:
-    """3x4 [R|T] world->camera of the ShapeNet renderer (az/el in degrees)."""
-    a, e = math.radians(-az_deg), math.radians(-el_deg)
-    sa, ca, se, ce = math.sin(a), math.cos(a), math.sin(e), math.cos(e)
+def blender_extrinsics(az_deg, el_deg, distance_ratio) -> np.ndarray:
+    """3x4 [R|T] world->camera of the ShapeNet renderer (az/el in degrees), float64.  The sines and the camera distance
+    are computed in the arguments' type, as getBlenderProj computes them: the view files pass the float32 values of
+    rendering_metadata.txt (disn_b200/create_img_h5.py), so there they are float32."""
+    a, e = np.radians(-az_deg), np.radians(-el_deg)
+    sa, ca, se, ce = np.sin(a), np.cos(a), np.sin(e), np.cos(e)
     world2obj = np.array([[ca * ce, -sa, ca * se],
                           [sa * ce, ca, sa * se],
                           [-se, 0.0, ce]], dtype=np.float64).T
@@ -46,7 +48,7 @@ def blender_extrinsics(az_deg: float, el_deg: float, distance_ratio: float) -> n
     obj2cam = cam_rot.T
     flip = np.diag([1.0, -1.0, -1.0])
     R = flip @ (obj2cam @ world2obj)
-    T = flip @ (-obj2cam @ np.array([[distance_ratio * CAM_MAX_DIST], [0.0], [0.0]]))
+    T = flip @ (-obj2cam @ np.array([[distance_ratio * CAM_MAX_DIST], [0.0], [0.0]], dtype=np.float64))
     return np.hstack([R, T])
 
 

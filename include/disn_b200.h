@@ -343,6 +343,22 @@ int disn_point_img_feat(disn_ctx* ctx, const float* pts, const float* trans_mat,
 int disn_eval_features(disn_ctx* ctx, const float* pts_rot, const float* global_feat, const float* point_feat, int32_t B,
                        int64_t N, float* out_pred, float* out_global, float* out_local, uint32_t flags);
 
+/* Checkpoint score at ground-truth samples, the metrics test/test_sdf_acc.py prints (models/model_normalization.py:
+ * 279-299, non-binary branch).  pts [B,N,3] (pts_rot = pts, as without --rot), trans_mat [B,4,3] and gt [B,N] (the
+ * loader's sdf_val) of the encoded batch; pred: NULL or [B,N], receiving pred_sdf bitwise equal to disn_eval_points's.
+ * With g = float32(gt - iso_offset) (the driver's sdf_val - 0.003) and p = pred, per image b:
+ *   count[b] = #{(g > 0) == (p > 0)};
+ *   wsum[b]  = float64 sum of |g * sdf_weight - p| * w, w = mask_weight if g <= 0.01 else 1;
+ *   rsum[b]  = float64 sum of |g - p / sdf_weight|;
+ * each term formed in float32 with correctly rounded operations in TF's order, the sums in a fixed order (repeated calls
+ * are bitwise equal).  Batch values: accuracy = float32(sum count) / float32(B*N), sdf_loss = float32(sum wsum / (B*N))
+ * * 1000 in float32, sdf_loss_realvalue = float32(sum rsum / (B*N)).  Host pointers (synchronous), or device pointers
+ * for every array with DISN_DEVICE_PTR (asynchronous; the DISN_PREC_F16F8 overflow status is then reported by the next
+ * synchronising call).  N >= 1, B = the encoded batch, sdf_weight non-zero, all three scalars finite. */
+int disn_sdf_metrics(disn_ctx* ctx, const float* pts, const float* trans_mat, const float* gt, int32_t B, int64_t N,
+                     float iso_offset, float sdf_weight, float mask_weight, uint32_t flags, float* pred, int64_t* count,
+                     double* wsum, double* rsum);
+
 /* Kernel launch counter (bench's gpu_launches): number of this library's kernels launched so far. */
 int64_t disn_launch_count(disn_ctx* ctx);
 
