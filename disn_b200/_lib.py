@@ -122,6 +122,7 @@ TEST_EXPORTS = {
     "disn_mesh_adaptive_bytes": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "disn_mesh_adaptive_edges": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
     "disn_debug_obj_tokens": (C.c_int, [C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "disn_debug_cam_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

@@ -402,7 +402,7 @@ int disn_cam_estimate(disn_ctx* c, const float* imgs, int32_t B, int32_t H, int3
   if (c->nn_scratch.ensure(carve(nullptr))) return -1;
   carve(c->nn_scratch.as<char>());
   DISN_CUDA_OK(cudaMemcpyAsync(dK, K ? K : kDefaultK, 9 * 4, cudaMemcpyHostToDevice, c->stream));
-  if (launch_cam_heads(c, B, dK, dRT, dTM)) return -1;
+  if (launch_cam_heads(c, B, c->emb.as<float>(), dK, dRT, dTM)) return -1;
   if (out_rt) DISN_CUDA_OK(cudaMemcpyAsync(out_rt, dRT, (size_t)B * 12 * 4, cudaMemcpyDeviceToHost, c->stream));
   DISN_CUDA_OK(cudaMemcpyAsync(out_trans_mat, dTM, (size_t)B * 12 * 4, cudaMemcpyDeviceToHost, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));

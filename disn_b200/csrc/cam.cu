@@ -5,6 +5,10 @@
 // y = relu(x.W + b), last layer linear), builds the rotation from the 6-D ortho representation, applies the
 // predicted isotropic scale, appends the translation row and right-multiplies by K^T:
 //     pred_RT[4,3] = [ (s*I).R ; t ],   pred_trans_mat[4,3] = pred_RT . K^T.
+// The pose geometry rounds every product, sum, square root and quotient to float32 on its own, like TF's separate ops:
+// this file is built with --fmad=false.  A contracted cross product x*y' - x'*y keeps the rounding error of one product,
+// so for y_raw parallel to x_raw it yields a residual of ~3e-8 instead of TF's exact zero, which the normalisation (clamp
+// 1e-8) then blows up into a unit z column pointing anywhere.  The heads' dot products use explicit fmaf (unaffected).
 #include "common.cuh"
 
 namespace disn {
@@ -70,24 +74,30 @@ __global__ void __launch_bounds__(256) cam_heads_kernel(const float* __restrict_
 
 }  // namespace
 
-int launch_cam_heads(disn_ctx* c, int B, const float* d_K, float* d_rt, float* d_tm) {
+int launch_cam_heads(disn_ctx* c, int B, const float* d_emb, const float* d_K, float* d_rt, float* d_tm) {
+  DISN_REQUIRE(c->cfg.num_classes <= 1024, "camera heads expect an embedding of at most 1024");
   CamHeadWeights w;
-  auto get = [&](const char* n, const float*& p) -> int {
-    auto it = c->weights.find(std::string("cameraprediction/") + n);
-    DISN_REQUIRE(it != c->weights.end(), std::string("missing variable cameraprediction/") + n);
+  // each variable must hold exactly the elements the kernel reads: [in, out] weights and [out] biases
+  auto get = [&](const char* n, int64_t numel, const float*& p) -> int {
+    const std::string name = std::string("cameraprediction/") + n;
+    auto it = c->weights.find(name);
+    DISN_REQUIRE(it != c->weights.end(), "missing variable " + name);
+    DISN_REQUIRE(it->second.numel == numel, "mis-shaped variable " + name);
     p = it->second.ptr();
     return 0;
   };
-  if (get("scale/fc1/weights", w.s1w) || get("scale/fc1/biases", w.s1b) || get("scale/fc2/weights", w.s2w) ||
-      get("scale/fc2/biases", w.s2b) || get("scale/fc3/weights", w.s3w) || get("scale/fc3/biases", w.s3b) ||
-      get("ortho6d/fc1/weights", w.r1w) || get("ortho6d/fc1/biases", w.r1b) || get("ortho6d/fc2/weights", w.r2w) ||
-      get("ortho6d/fc2/biases", w.r2b) || get("ortho6d/fc3/weights", w.r3w) || get("ortho6d/fc3/biases", w.r3b) ||
-      get("translation/fc1/weights", w.t1w) || get("translation/fc1/biases", w.t1b) ||
-      get("translation/fc2/weights", w.t2w) || get("translation/fc2/biases", w.t2b) ||
-      get("translation/fc3/weights", w.t3w) || get("translation/fc3/biases", w.t3b))
+  const int64_t e = c->cfg.num_classes;
+  if (get("scale/fc1/weights", e * 64, w.s1w) || get("scale/fc1/biases", 64, w.s1b) ||
+      get("scale/fc2/weights", 64 * 32, w.s2w) || get("scale/fc2/biases", 32, w.s2b) ||
+      get("scale/fc3/weights", 32, w.s3w) || get("scale/fc3/biases", 1, w.s3b) ||
+      get("ortho6d/fc1/weights", e * 512, w.r1w) || get("ortho6d/fc1/biases", 512, w.r1b) ||
+      get("ortho6d/fc2/weights", 512 * 256, w.r2w) || get("ortho6d/fc2/biases", 256, w.r2b) ||
+      get("ortho6d/fc3/weights", 256 * 6, w.r3w) || get("ortho6d/fc3/biases", 6, w.r3b) ||
+      get("translation/fc1/weights", e * 128, w.t1w) || get("translation/fc1/biases", 128, w.t1b) ||
+      get("translation/fc2/weights", 128 * 64, w.t2w) || get("translation/fc2/biases", 64, w.t2b) ||
+      get("translation/fc3/weights", 64 * 3, w.t3w) || get("translation/fc3/biases", 3, w.t3b))
     return -2;
-  DISN_REQUIRE(c->cfg.num_classes <= 1024, "camera heads expect an embedding of at most 1024");
-  cam_heads_kernel<<<B, 256, 0, c->stream>>>(c->emb.as<float>(), c->cfg.num_classes, w, d_K, d_rt, d_tm);
+  cam_heads_kernel<<<B, 256, 0, c->stream>>>(d_emb, c->cfg.num_classes, w, d_K, d_rt, d_tm);
   c->launches++;
   DISN_CUDA_OK(cudaGetLastError());
   return 0;

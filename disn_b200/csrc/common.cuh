@@ -354,7 +354,8 @@ int conv_tc_pack(disn_ctx* c, const float* d_w, int K, int N, DevBuffer& out);
 int launch_conv_tc(disn_ctx* c, const float* A, const uint8_t* wpk, const float* bias, float* C, float* ws,
                    int64_t ws_elems, int M, int N, int K, int H, int W, int Cin, int relu, int* splits_out);
 // cam.cu
-int launch_cam_heads(disn_ctx* c, int B, const float* d_K, float* d_rt, float* d_tm);
+// the pose heads on the embeddings d_emb [B, num_classes] (device) -> pred_RT and pred_trans_mat [B,4,3] (device)
+int launch_cam_heads(disn_ctx* c, int B, const float* d_emb, const float* d_K, float* d_rt, float* d_tm);
 // chamfer.cu
 int nn_distance(disn_ctx* c, const float* d_xyz1, int n, const float* d_xyz2, int m, int B, float* d_dist1,
                 int* d_idx1, float* d_dist2, int* d_idx2);

@@ -61,6 +61,11 @@ int disn_mesh_adaptive_edges(disn_ctx* ctx, int64_t first, int64_t n, int64_t* o
  * it.  Needs no device. */
 int disn_debug_obj_tokens(const char* text, const int64_t* offsets, const int32_t* lengths, int64_t n, float* out);
 
+/* Diagnostic: the camera-pose heads of disn_cam_estimate on a caller's embedding emb [B, num_classes] (host) instead of
+ * the encoder's; K [3,3] row-major (NULL = the default intrinsics) -> out_rt and out_trans_mat [B,4,3] (host).  The
+ * context's encoder products are left as they are. */
+int disn_debug_cam_heads(disn_ctx* ctx, const float* emb, int32_t B, const float* K, float* out_rt, float* out_trans_mat);
+
 #ifdef __cplusplus
 }
 #endif

@@ -414,3 +414,87 @@ def cam_estimate(imgs, W, K=CAM_K, dtype=np.float64):
     Rs = scale @ R
     RT = np.concatenate([Rs, t[:, None, :]], axis=1)
     return RT, RT @ np.asarray(K, dtype).T
+
+
+# Faults cam_pose can apply, so a test can show each one is visible to the camera tests' bounds.
+CAM_FAULTS = ("offset_dropped", "offset_permuted", "K_not_transposed", "rows_not_columns", "z_unnormalised",
+              "no_clamp", "scale_after_translation")
+
+
+def cam_head_outputs(emb, W, mode="float64"):
+    """The three fully-connected heads of posenet.get_cam_mat on embeddings [B, num_classes] -> (scale [B],
+    ortho6d [B,6], translation [B,3]) before the offset.  "float64": float64 throughout; "float32-ops": the same float64
+    values rounded once to float32 (a correctly rounded dot product: TF's float32 matmul pins no summation order)."""
+    g = np.asarray(emb, np.float64)
+
+    def head(name):
+        h = g
+        for i in (1, 2, 3):
+            h = h @ np.asarray(W["cameraprediction/%s/fc%d/weights" % (name, i)], np.float64) + \
+                np.asarray(W["cameraprediction/%s/fc%d/biases" % (name, i)], np.float64)
+            if i < 3:
+                h = np.maximum(h, 0)
+        return h
+
+    out = head("scale")[:, 0], head("ortho6d"), head("translation")
+    return tuple(o.astype(np.float32) for o in out) if mode == "float32-ops" else out
+
+
+def cam_pose(scale, ortho6d, translation, K=CAM_K, mode="float64", fault=None):
+    """posenet.get_cam_mat after its heads (posenet.py:97,120-124, :13-36) and model_cam.py:102-103 -> (pred_RT [B,4,3],
+    pred_trans_mat [B,4,3]).  "float64": every op in float64.  "float32-ops": every TF op rounded to float32 on its own,
+    in TF's order -- square, reduce_sum (left to right), sqrt, maximum(., 1e-8), divide, cross (each product, then the
+    difference), scale * I, matmul(scale * I, R), + offset, matmul(RT, K^T) (products, then left-to-right sums).
+    `fault` (one of CAM_FAULTS) applies a deliberate mistake instead of the reference's step."""
+    f = np.float32 if mode == "float32-ops" else np.float64
+    assert mode in ("float64", "float32-ops") and (fault is None or fault in CAM_FAULTS)
+    s = np.asarray(scale, f).reshape(-1)
+    p = np.asarray(ortho6d, f)
+    t = np.asarray(translation, f)
+    Km = np.asarray(K, f).reshape(3, 3)
+    B = s.shape[0]
+
+    def normalize(v):
+        sq = v * v
+        mag = np.sqrt((sq[:, 0] + sq[:, 1]) + sq[:, 2])[:, None]
+        if fault != "no_clamp":
+            mag = np.maximum(mag, f(1e-8))
+        with np.errstate(invalid="ignore", divide="ignore"):
+            return v / mag
+
+    def cross(a, b):
+        return np.stack([a[:, 1] * b[:, 2] - a[:, 2] * b[:, 1], a[:, 2] * b[:, 0] - a[:, 0] * b[:, 2],
+                         a[:, 0] * b[:, 1] - a[:, 1] * b[:, 0]], axis=1)
+
+    with np.errstate(over="ignore", invalid="ignore"):
+        x = normalize(p[:, 0:3])
+        z = cross(x, p[:, 3:6])
+        if fault != "z_unnormalised":
+            z = normalize(z)
+        y = cross(z, x)
+        R = np.stack([x, y, z], axis=1 if fault == "rows_not_columns" else 2)     # matrix[:, i, j] = (x, y, z)[j][i]
+        S = s[:, None, None] * np.eye(3, dtype=f)[None]
+        off = np.asarray(CAM_T_OFFSET, f)
+        if fault == "offset_dropped":
+            off = np.zeros(3, f)
+        elif fault == "offset_permuted":
+            off = off[[1, 2, 0]]
+        tr = (t + off)[:, None, :]
+
+        def matmul(A, Bm):          # [B,n,3] @ [3,m] or [B,3,m]: each product rounded, summed left to right
+            Bm = np.broadcast_to(Bm, (A.shape[0],) + Bm.shape[-2:])
+            return (A[:, :, 0, None] * Bm[:, None, 0, :] + A[:, :, 1, None] * Bm[:, None, 1, :]) + \
+                A[:, :, 2, None] * Bm[:, None, 2, :]
+
+        if fault == "scale_after_translation":
+            RT = s[:, None, None] * np.concatenate([R, tr], axis=1)
+        else:
+            RT = np.concatenate([matmul(S, R), tr], axis=1)
+        TM = matmul(RT, Km if fault == "K_not_transposed" else Km.T)
+    assert RT.dtype == f and TM.dtype == f and RT.shape == (B, 4, 3)
+    return RT, TM
+
+
+def cam_heads(emb, W, K=CAM_K, mode="float64", fault=None):
+    """model_cam.get_model's camera branch (non-shift) on given embeddings [B, num_classes] instead of the VGG's."""
+    return cam_pose(*cam_head_outputs(emb, W, mode), K=K, mode=mode, fault=fault)
