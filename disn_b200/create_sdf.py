@@ -89,7 +89,8 @@ def create(weights, batches, device=0):
     is_training_pl = model.Placeholder("is_training", ())
     end_points = model.get_model(input_pls, NUM_POINTS, is_training_pl, bn=False, FLAGS=FLAGS)
     loss, end_points = model.get_loss(end_points, sdf_weight=SDF_WEIGHT, num_sample_points=NUM_SAMPLE_POINTS, FLAGS=FLAGS)
-    sess = model.Session(device=device, precision=getattr(FLAGS, "precision", "f16f8"), max_batch=max(1, BATCH_SIZE))
+    sess = model.Session(device=device, precision=getattr(FLAGS, "precision", "f16f8"), max_batch=max(1, BATCH_SIZE),
+                         img_h=FLAGS.img_h, img_w=FLAGS.img_w)
     if weights is None:
         print("Fail to load overall modelfile: %s" % LOG_DIR)       # create_sdf.py:192
         raise RuntimeError("no weights supplied: pass the checkpoint variables (or a random init) explicitly")

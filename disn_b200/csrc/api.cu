@@ -50,6 +50,10 @@ int disn_create(const disn_config* cfg, disn_ctx** out) {
   DISN_REQUIRE(cfg && out, "null config/out");
   DISN_REQUIRE(cfg->max_batch >= 1 && cfg->max_batch <= 8, "max_batch in [1,8]");
   DISN_REQUIRE(cfg->img_h > 1 && cfg->img_w > 1 && cfg->num_classes % 4 == 0, "bad image/embedding size");
+  // the tensor-core point kernel addresses one image's projected map with 32-bit element offsets (point_tc.cu taps_of)
+  DISN_REQUIRE((int64_t)cfg->img_h * cfg->img_w * kHidden < ((int64_t)1 << 31),
+               "feature map too large: img_h * img_w * 512 must stay below 2^31 (" + std::to_string(cfg->img_h) + " x " +
+                   std::to_string(cfg->img_w) + " given)");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev == 0) {

@@ -27,19 +27,28 @@ class MeshCleanCounts(NamedTuple):
     n_kept: int
 
 
+def engine_config(device: int = 0, precision: str = "fp32", max_batch: int = 1, tanh: bool = False,
+                  img_h: int = 137, img_w: int = 137, num_classes: int = 1024, sdf_weight: float = 10.0) -> DisnConfig:
+    """The disn_config an Engine with these arguments is created with (no device needed)."""
+    cfg = DisnConfig()
+    _lib.load().disn_default_config(C.byref(cfg))
+    cfg.device = device
+    cfg.precision = _PREC[precision]
+    cfg.max_batch = max_batch
+    cfg.tanh_out = int(bool(tanh))
+    cfg.img_h, cfg.img_w, cfg.num_classes = img_h, img_w, num_classes
+    cfg.sdf_weight = sdf_weight
+    # models/model_normalization.py:249-251 clamps projected points to the constant [0, 136] whatever FLAGS.img_h/img_w
+    # are: on a smaller map the points beyond its edge get no features, on a larger one nothing is read beyond 136
+    cfg.clamp_max = 136.0
+    return cfg
+
+
 class Engine:
     def __init__(self, device: int = 0, precision: str = "fp32", max_batch: int = 1, tanh: bool = False,
                  img_h: int = 137, img_w: int = 137, num_classes: int = 1024, sdf_weight: float = 10.0):
         self.lib = _lib.load()
-        cfg = DisnConfig()
-        self.lib.disn_default_config(C.byref(cfg))
-        cfg.device = device
-        cfg.precision = _PREC[precision]
-        cfg.max_batch = max_batch
-        cfg.tanh_out = int(bool(tanh))
-        cfg.img_h, cfg.img_w, cfg.num_classes = img_h, img_w, num_classes
-        cfg.sdf_weight = sdf_weight
-        cfg.clamp_max = float(img_h - 1)      # models/model_normalization.py:250 (136 for 137x137)
+        cfg = engine_config(device, precision, max_batch, tanh, img_h, img_w, num_classes, sdf_weight)
         self.cfg = cfg
         self._h = C.c_void_p()
         check(self.lib.disn_create(C.byref(cfg), C.byref(self._h)))

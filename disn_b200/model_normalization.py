@@ -149,17 +149,40 @@ class Session:
     """Plays tf.Session for the hot path.  ``weights``: dict TF-variable-name -> array (the checkpoint
     contract, SURVEY.md 8a); like the reference's restore (test/create_sdf.py:186-192) missing variables are
     tolerated only in the sense that whatever was loaded is used -- the encoder refuses to run without its
-    weights rather than silently using zeros."""
+    weights rather than silently using zeros.
 
-    def __init__(self, weights=None, device=0, precision="bf16x3", max_batch=8, engine=None):
-        self.engine = engine or Engine(device=device, precision=precision, max_batch=max_batch)
+    The feature maps are img_h x img_w (FLAGS.img_h / img_w of the graph).  A Session that built its own engine rebuilds
+    it, with the weights it was given, when run() meets a graph of another map size; one given an engine of another size
+    refuses the graph."""
+
+    def __init__(self, weights=None, device=0, precision="bf16x3", max_batch=8, engine=None, img_h=137, img_w=137):
+        self._own = engine is None
+        self._args = dict(device=device, precision=precision, max_batch=max_batch)
+        self.engine = engine or Engine(img_h=img_h, img_w=img_w, **self._args)
         self._img_key = None
+        self._weights = None
         if weights is not None:
-            self.engine.load_weights(weights)
+            self.load_weights(weights)
 
     def load_weights(self, weights):
         self.engine.load_weights(weights)
+        self._weights = weights
         self._img_key = None
+
+    def _fit_map_size(self, FLAGS):
+        """Make the engine's feature maps FLAGS.img_h x FLAGS.img_w (model_normalization.py:171-183 resizes to them)."""
+        size = (int(FLAGS.img_h), int(FLAGS.img_w))
+        have = (self.engine.cfg.img_h, self.engine.cfg.img_w)
+        if size == have:
+            return
+        if not self._own:
+            raise ValueError("the graph's FLAGS.img_h x img_w is %d x %d but the Session's engine holds %d x %d feature "
+                             "maps: build the Engine with img_h=%d, img_w=%d" % (size + have + size))
+        self.engine.close()
+        self.engine = Engine(img_h=size[0], img_w=size[1], **self._args)
+        self._img_key = None
+        if self._weights is not None:
+            self.engine.load_weights(self._weights)
 
     def close(self):
         self.engine.close()
@@ -178,6 +201,8 @@ class Session:
         if graph is None:
             raise ValueError("nothing to run")
         pl = graph.pl
+        if graph.FLAGS is not None:
+            self._fit_map_size(graph.FLAGS)
         imgs = self._feed(feed_dict, pl.get("imgs"))
         pts = self._feed(feed_dict, pl.get("sample_pc"))
         rot = self._feed(feed_dict, pl.get("sample_pc_rot"))

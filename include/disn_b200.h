@@ -70,10 +70,12 @@ enum {
 
 typedef struct disn_config {
   int32_t device;        /* CUDA device ordinal */
-  int32_t img_h, img_w;  /* FLAGS.img_h / img_w (137): size the feature taps are resized to */
+  int32_t img_h, img_w;  /* FLAGS.img_h / img_w (137): size the feature taps are resized to;
+                            disn_create refuses img_h * img_w * 512 >= 2^31 */
   int32_t vgg_in;        /* get_model img_size (224) */
   int32_t num_classes;   /* FLAGS.num_classes (1024): width of the global embedding */
-  float clamp_max;       /* 136.0: upper clamp of projected pixel coordinates */
+  float clamp_max;       /* 136.0: upper clamp of projected pixel coordinates (the reference's constant, whatever
+                            img_h / img_w are) */
   float sdf_weight;      /* SDF_WEIGHT (10.0): eval_grid divides by it */
   int32_t tanh_out;      /* FLAGS.tanh */
   int32_t precision;     /* DISN_PREC_* */

@@ -61,3 +61,27 @@ def test_default_config_values():
     lib.disn_default_config(C.byref(cfg))
     assert (cfg.img_h, cfg.img_w, cfg.vgg_in, cfg.num_classes) == (137, 137, 224, 1024)
     assert cfg.clamp_max == 136.0 and cfg.sdf_weight == 10.0 and cfg.tanh_out == 0
+
+
+@pytest.mark.parametrize("hw", [(137, 137), (64, 64), (128, 128), (137, 173), (173, 137), (256, 256)])
+def test_engine_config_clamps_at_136_whatever_the_map_size(hw):
+    """models/model_normalization.py:249-251 clamps projections to the constant [0, 136]; the map size only sets the
+    size the taps are resized to."""
+    from disn_b200.engine import engine_config
+    cfg = engine_config(img_h=hw[0], img_w=hw[1], precision="f16f8", max_batch=2)
+    assert (cfg.img_h, cfg.img_w) == hw and cfg.clamp_max == 136.0
+    assert (cfg.precision, cfg.max_batch, cfg.vgg_in) == (2, 2, 224)
+
+
+@pytest.mark.parametrize("hw", [(2048, 2048), (2049, 2049), (2, 2 ** 30), (65536, 65536)])
+def test_create_refuses_a_map_of_2_31_elements_before_touching_a_device(hw):
+    """The tensor-core point kernel addresses one image's [img_h, img_w, 512] map with 32-bit offsets: disn_create
+    refuses img_h * img_w * 512 >= 2^31 before it looks for a device (so also on a machine without one) and names the
+    limit.  65536 x 65536 would wrap a 32-bit product to 0."""
+    from disn_b200 import _lib
+    from disn_b200.engine import engine_config
+    lib = _lib.load()
+    h = C.c_void_p()
+    cfg = engine_config(img_h=hw[0], img_w=hw[1])
+    assert lib.disn_create(C.byref(cfg), C.byref(h)) != 0 and not h.value
+    assert "img_h * img_w * 512 must stay below 2^31" in lib.disn_last_error().decode()

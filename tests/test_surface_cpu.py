@@ -41,6 +41,21 @@ def test_out_of_scope_branches_are_refused_loudly(flag):
         model.get_model(pls, 1, None, FLAGS=F)
 
 
+def test_session_refuses_a_graph_of_another_map_size_than_its_engine():
+    """A Session given an engine of one feature-map size refuses a graph whose FLAGS.img_h / img_w ask for another,
+    instead of running it silently on the engine's maps (tests/test_gpu_map_sizes.py covers the engine it builds)."""
+    from disn_b200 import model_normalization as model
+    eng = SimpleNamespace(cfg=SimpleNamespace(img_h=137, img_w=137))
+    sess = model.Session(engine=eng)
+    for hw in ((128, 128), (137, 173)):
+        F = _flags(img_h=hw[0], img_w=hw[1])
+        pls = model.placeholder_inputs(1, 1, (137, 137), num_sample_pc=8, FLAGS=F)
+        ep = model.get_model(pls, 1, None, FLAGS=F)
+        with pytest.raises(ValueError, match=r"%d x %d but the Session's engine holds 137 x 137" % hw):
+            sess.run(ep["pred_sdf"], feed_dict={pls["imgs"]: np.zeros((1, 137, 137, 3), np.float32)})
+    assert sess.engine is eng
+
+
 def test_driver_constants_match_reference_arithmetic(golden, tmp_path):
     from disn_b200 import create_sdf as cs
     for sdf_res, R, total, split, nsp in golden["chunking"]["table"]:

@@ -41,6 +41,37 @@ def test_exact_mode_equals_the_float64_oracle(he_weights, tanh):
     assert (u >= H - 1).any() and (u < H - 1).mean() > 0.5        # inside, on the last column's far taps and past them
 
 
+@pytest.mark.parametrize("hw", [(24, 40), (40, 24)])
+def test_exact_mode_equals_the_float64_oracle_on_a_non_square_map(he_weights, hw):
+    """The same on img_h != img_w maps, resized from the taps the way FLAGS.img_h / img_w select, with the projection
+    run past both far edges and the constant clamp at 136 beyond them: pins u to img_w and v to img_h in the emulation's
+    gather, so that tests/test_gpu_map_sizes.py can lean on it at non-square map sizes."""
+    H, W = hw
+    F = orc.default_flags(img_h=H, img_w=W)
+    rng = np.random.default_rng(5)
+    maps = [orc.tf_resize_bilinear(rng.standard_normal((1, 17, 17, c)) * 0.5, F.img_h, F.img_w, np.float64)
+            for c in orc.TAP_CHANNELS]
+    emb = rng.standard_normal((1, 1024))
+    tm = synth.DEMO_TRANS_MAT.astype(np.float64) * np.array([(W + 6) / 137.0, (H + 6) / 137.0, 1.0])
+    pts = rng.uniform(-1.3, 1.3, size=(1, 900, 3)).astype(np.float32)
+    pts[0, :100] *= 8.0                     # far outside: projections clamped to 0 and to 136
+    Wg = np.asarray(he_weights["sdfprediction/fold2/conv1/weights"], np.float64).reshape(-1, 512)
+    Wl = np.asarray(he_weights["sdfprediction_imgfeat/fold2/conv1/weights"], np.float64).reshape(-1, 512)
+    gbias = emb @ Wg[512:] + np.asarray(he_weights["sdfprediction/fold2/conv1/biases"], np.float64)
+    offs = np.cumsum([512] + list(orc.TAP_CHANNELS[:-1]))
+    pmap = sum(m @ Wl[o:o + c] for m, o, c in zip(maps, offs, orc.TAP_CHANNELS))
+    assert pmap.shape == (1, H, W, 512)
+    ref = orc.decode(SimpleNamespace(img_embedding=emb, maps=maps), pts, pts, tm, he_weights, FLAGS=F, dtype=np.float64)
+    got = te.emulate(he_weights, pts, tm, pmap, gbias, "exact")
+    assert np.abs(got["pred"] - ref["pred_sdf"][..., 0]).max() <= 1e-12
+    assert np.abs(got["local"] - ref["pred_sdf_value_local"][..., 0]).max() <= 1e-12
+    assert np.abs(got["uv"] - ref["sample_img_points"]).max() <= 1e-12
+    u, v = got["uv"][0, :, 0], got["uv"][0, :, 1]
+    for x, n in ((u, W), (v, H)):           # inside, between the last texel and the map's edge, past it, clamped
+        assert ((x > 1) & (x < n - 1)).mean() > 0.3 and ((x > n - 1) & (x < n)).any() and ((x >= n) & (x < 136)).any()
+        assert (x == 136).any() and (x == 0).any()
+
+
 def test_exact_mode_streams_equal_the_oracle_streams(he_weights):
     rng = np.random.default_rng(4)
     maps = [rng.standard_normal((1, 20, 20, c)) * 0.5 for c in orc.TAP_CHANNELS]
