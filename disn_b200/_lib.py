@@ -64,6 +64,7 @@ EXPORTS = {
     "disn_mc_run": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_float, C.c_uint32,
                               C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "disn_mc_fetch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "disn_mesh_counts": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "disn_mc_write_obj": (C.c_int, [C.c_void_p, C.c_char_p]),
     "disn_mesh_load": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]),
     "disn_mesh_clean": (C.c_int, [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.POINTER(C.c_int64),

@@ -73,8 +73,7 @@ int disn_mesh_adaptive_from_field(disn_ctx* c, const float* field, int32_t sdf_r
                                  c->stream));
     d = c->ad_field.as<float>();
   }
-  const int rc = adaptive_mesh_run(c, d, 0, nullptr, sdf_res, sdf_params, iso, band, level_counts, n_levels, nullptr,
-                                   nullptr);
+  const int rc = adaptive_mesh_run(c, d, 0, nullptr, sdf_res, sdf_params, iso, band, level_counts, n_levels);
   return finish_mesh_call(c, rc, n_verts, n_faces);
 }
 

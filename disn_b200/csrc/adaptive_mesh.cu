@@ -215,8 +215,7 @@ size_t adaptive_mesh_bytes(const disn_ctx* c) {
 }
 
 int adaptive_mesh_run(disn_ctx* c, const float* field, int image, const float* d_tm, int32_t res, const double* sdf_params,
-                      float iso, double band, int64_t* level_counts, int32_t* n_levels, int64_t* n_verts,
-                      int64_t* n_faces) {
+                      float iso, double band, int64_t* level_counts, int32_t* n_levels) {
   cudaStream_t st = c->stream;
   const int R = res + 1;
   c->am_nv = -1;
@@ -295,25 +294,20 @@ int adaptive_mesh_run(disn_ctx* c, const float* field, int image, const float* d
     unsigned long long* edges = nullptr;
     if (sort_keys(c, c->am_edges, nv, key_bits((unsigned long long)R * R * R * 3), &edges)) return -1;
     c->am_edges_sorted = edges;
-    c->mc_nv = c->mc_nf = 0;                               // the resident mesh is replaced from here on
-    if (ensure_mesh(c->mc_verts, c->mc_faces, nv, nf)) return -1;
+    if (c->mesh.replace(nv, nf)) return -1;
     Geom g;
     for (int k = 0; k < 3; ++k) { g.lo[k] = sdf_params[k]; g.h[k] = (sdf_params[3 + k] - sdf_params[k]) / (double)(R - 1); }
-    vertices_kernel<<<blocks_of(nv), AM_THREADS, 0, st>>>(f, g, edges, nv, c->mc_verts.as<float>());
-    faces_kernel<<<blocks_of(n_cells), AM_THREADS, 0, st>>>(cells, n_cells, R, cases, foff, edges, nv,
-                                                            c->mc_faces.as<int32_t>());
+    vertices_kernel<<<blocks_of(nv), AM_THREADS, 0, st>>>(f, g, edges, nv, c->mesh.verts());
+    faces_kernel<<<blocks_of(n_cells), AM_THREADS, 0, st>>>(cells, n_cells, R, cases, foff, edges, nv, c->mesh.faces());
     c->launches += 2;
     DISN_CUDA_OK(cudaGetLastError());
-  } else {
-    c->mc_nv = c->mc_nf = 0;
-    if (ensure_mesh(c->mc_verts, c->mc_faces, 0, 0)) return -1;
+  } else if (c->mesh.replace(0, 0)) {
+    return -1;
   }
   DISN_CUDA_OK(cudaEventRecord(c->am_ev[3], st));
   DISN_CUDA_OK(cudaStreamSynchronize(st));
-  c->mc_nv = nv; c->mc_nf = nf;
+  c->mesh.commit(nv, nf);
   c->am_nv = nv;
-  if (n_verts) *n_verts = nv;
-  if (n_faces) *n_faces = nf;
   return 0;
 }
 

@@ -476,25 +476,35 @@ int disn_mc_run(disn_ctx* c, const float* sdf, int32_t R, const double* bbox, fl
                 int64_t* n_verts, int64_t* n_faces) {
   DISN_REQUIRE(c && sdf && bbox, "null argument");
   DISN_REQUIRE(R >= 2, "need at least 2 samples per axis");
+  DISN_REQUIRE((int64_t)R * R * R * 3 < (int64_t)1 << 32, "grid too large for 32-bit vertex ids");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
   const float* d_sdf = nullptr;
-  if (mc_input(c, sdf, R, flags, &d_sdf)) return -1;
-  return mc_run(c, d_sdf, R, bbox, iso, n_verts, n_faces);
+  int rc = mc_input(c, sdf, R, flags, &d_sdf);
+  if (!rc) rc = mc_run(c, d_sdf, R, bbox, iso);
+  return finish_mesh_call(c, rc, n_verts, n_faces);
 }
 
 int disn_mc_fetch(disn_ctx* c, float* verts, int32_t* faces) {
   DISN_REQUIRE(c, "null ctx");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
-  return mc_fetch(c, verts, faces);
+  return c->mesh.fetch(c->stream, verts, faces);
+}
+
+int disn_mesh_counts(disn_ctx* c, int64_t* n_verts, int64_t* n_faces) {
+  DISN_REQUIRE(c && n_verts && n_faces, "null argument");
+  *n_verts = c->mesh.nv();
+  *n_faces = c->mesh.nf();
+  return 0;
 }
 
 int disn_mc_write_obj(disn_ctx* c, const char* path) {
   DISN_REQUIRE(c && path, "null argument");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
-  std::vector<float> v((size_t)c->mc_nv * 3);
-  std::vector<int32_t> f((size_t)c->mc_nf * 3);
-  if (mc_fetch(c, v.data(), f.data())) return -1;
-  return disn_write_obj(path, v.data(), c->mc_nv, f.data(), c->mc_nf);
+  const int64_t nv = c->mesh.nv(), nf = c->mesh.nf();
+  std::vector<float> v((size_t)nv * 3);
+  std::vector<int32_t> f((size_t)nf * 3);
+  if (c->mesh.fetch(c->stream, v.data(), f.data())) return -1;
+  return disn_write_obj(path, v.data(), nv, f.data(), nf);
 }
 
 int disn_marching_cubes(disn_ctx* c, const float* sdf, int32_t R, const double* bbox, float iso, float* verts,
@@ -506,13 +516,20 @@ int disn_marching_cubes(disn_ctx* c, const float* sdf, int32_t R, const double* 
   if (verts == nullptr || faces == nullptr) { *n_verts = nv; *n_faces = nf; return 0; }     // counting call
   if (*n_verts < nv || *n_faces < nf) { set_error("marching_cubes: output buffers too small"); return -2; }
   *n_verts = nv; *n_faces = nf;
-  return mc_fetch(c, verts, faces);
+  return c->mesh.fetch(c->stream, verts, faces);
 }
 
 int disn_mesh_load(disn_ctx* c, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces) {
   DISN_REQUIRE(c, "null ctx");
+  DISN_REQUIRE(n_verts >= 0 && n_faces >= 0 && (verts || n_verts == 0) && (faces || n_faces == 0),
+               "bad mesh_load arguments");
+  DISN_REQUIRE(n_verts < ((int64_t)1 << 31) && 3 * n_faces < ((int64_t)1 << 31), "mesh too large for 32-bit indices");
+  for (int64_t i = 0; i < 3 * n_faces; ++i)
+    if (faces[i] < 0 || faces[i] >= n_verts)
+      DISN_REQUIRE(false, "face " + std::to_string(i / 3) + " references vertex " + std::to_string(faces[i]) +
+                              " outside [0, " + std::to_string(n_verts) + ")");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
-  return mesh_load(c, verts, n_verts, faces, n_faces);
+  return finish_mesh_call(c, mesh_load(c, verts, n_verts, faces, n_faces), nullptr, nullptr);
 }
 
 int disn_mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
@@ -667,11 +684,11 @@ int disn_eval_grid_adaptive(disn_ctx* c, const double* sdf_params, const float* 
 // what disn_mc_fetch copies.
 int disn::finish_mesh_call(disn_ctx* c, int rc, int64_t* n_verts, int64_t* n_faces) {
   if (rc) {
-    c->mc_nv = c->mc_nf = 0;
+    c->mesh.clear();
     c->am_nv = -1;
   }
-  if (n_verts) *n_verts = c->mc_nv;
-  if (n_faces) *n_faces = c->mc_nf;
+  if (n_verts) *n_verts = c->mesh.nv();
+  if (n_faces) *n_faces = c->mesh.nf();
   return rc;
 }
 
@@ -700,10 +717,9 @@ int disn_mesh_grid_adaptive(disn_ctx* c, const double* sdf_params, const float* 
     c->am_nv = -1;                              // the mesher's diagnostics describe no call until its next one
     c->am_edges_sorted = nullptr;
     rc = adaptive_run(c, nullptr, image, c->d_tm.as<float>(), sdf_res, sdf_params, iso, band, level_counts, n_levels);
-    if (!rc) rc = mc_run(c, c->ad_grid.as<float>(), (int)R, sdf_params, iso, nullptr, nullptr);
+    if (!rc) rc = mc_run(c, c->ad_grid.as<float>(), (int)R, sdf_params, iso);
   } else if (!rc) {
-    rc = adaptive_mesh_run(c, nullptr, image, c->d_tm.as<float>(), sdf_res, sdf_params, iso, band, level_counts, n_levels,
-                           nullptr, nullptr);
+    rc = adaptive_mesh_run(c, nullptr, image, c->d_tm.as<float>(), sdf_res, sdf_params, iso, band, level_counts, n_levels);
   }
   if (!rc && cudaStreamSynchronize(c->stream) != cudaSuccess) {
     set_error("mesh_grid_adaptive: stream synchronisation failed");

@@ -215,6 +215,57 @@ __device__ __forceinline__ void project(const float* T, float clamp_max, float x
   v = fminf(clamp_max, fmaxf(0.f, q1 / q2));
 }
 
+// The device-resident mesh the mesh calls share: vertices [nv,3] float32 and faces [nf,3] int32 (0-based), plus a spare
+// pair that cleaning compacts into.  The counts always describe arrays that are allocated and written: a writer calls
+// replace(), which empties the mesh before it makes room, writes through verts() / faces() and then commit()s the counts,
+// so a writer that fails in between leaves the empty mesh.  The arrays grow only, with 25 % + 1024 elements of slack.
+class ResidentMesh {
+ public:
+  int64_t nv() const { return nv_; }
+  int64_t nf() const { return nf_; }
+  float* verts() const { return verts_.as<float>(); }
+  int32_t* faces() const { return faces_.as<int32_t>(); }
+
+  int replace(int64_t nv, int64_t nf) {
+    clear();
+    return grow(verts_, faces_, nv, nf);
+  }
+  void commit(int64_t nv, int64_t nf) { nv_ = nv; nf_ = nf; }
+  void clear() { nv_ = nf_ = 0; }
+
+  // room for a mesh built from the resident one; the resident mesh is untouched until swap_spare makes the spare pair
+  // resident with the given counts
+  int reserve_spare(int64_t nv, int64_t nf) { return grow(spare_verts_, spare_faces_, nv, nf); }
+  float* spare_verts() const { return spare_verts_.as<float>(); }
+  int32_t* spare_faces() const { return spare_faces_.as<int32_t>(); }
+  void swap_spare(int64_t nv, int64_t nf) {
+    std::swap(verts_, spare_verts_);
+    std::swap(faces_, spare_faces_);
+    commit(nv, nf);
+  }
+
+  // copies the mesh to host arrays of nv()*3 floats / nf()*3 int32 (an array is copied only when the mesh has entries
+  // of its kind and its pointer is non-null) on `stream`, then synchronises with it
+  int fetch(cudaStream_t stream, float* verts, int32_t* faces) const {
+    if (nv_ && verts)
+      DISN_CUDA_OK(cudaMemcpyAsync(verts, verts_.as<float>(), (size_t)nv_ * 3 * sizeof(float), cudaMemcpyDeviceToHost,
+                                   stream));
+    if (nf_ && faces)
+      DISN_CUDA_OK(cudaMemcpyAsync(faces, faces_.as<int32_t>(), (size_t)nf_ * 3 * sizeof(int32_t),
+                                   cudaMemcpyDeviceToHost, stream));
+    DISN_CUDA_OK(cudaStreamSynchronize(stream));
+    return 0;
+  }
+
+ private:
+  static int grow(DevBuffer& verts, DevBuffer& faces, int64_t nv, int64_t nf) {
+    const size_t vb = 3 * sizeof(float), fb = 3 * sizeof(int32_t);
+    return verts.ensure(nv * vb, (nv / 4 + 1024) * vb) || faces.ensure(nf * fb, (nf / 4 + 1024) * fb) ? -1 : 0;
+  }
+  DevBuffer verts_, faces_, spare_verts_, spare_faces_;
+  int64_t nv_ = 0, nf_ = 0;
+};
+
 }  // namespace disn
 
 // Every allocation of the context is a buffer member: deleting the context frees them all.
@@ -260,15 +311,15 @@ struct disn_ctx {
   disn::DevBuffer tc_weights_f8;       // fp16 + e5m2 stage images (DISN_PREC_F16F8)
   float tc_act_scale[2][4][2] = {};
   std::map<std::string, disn::DevBuffer> enc_tc_weights;   // packed bf16 hi/lo stage images of the encoder GEMMs
-  // marching cubes: persistent scratch + the device-resident mesh of the last run (mc.cu)
+  // the mesh that marching cubes, the coarse-to-fine mesher, mesh_load and the OBJ reader write and the other mesh calls
+  // read or change in place
+  disn::ResidentMesh mesh;
+  // marching cubes: persistent scratch (mc.cu)
   disn::DevBuffer mc_code, mc_vbase, mc_chunk, mc_sums, mc_totals;
   disn::PinnedBuffer mc_totals_host;
-  disn::DevBuffer mc_verts, mc_faces;
-  int64_t mc_nv = 0, mc_nf = 0;
-  // small-part cleaning of the resident mesh (mesh_clean.cu): scratch arena, the compacted mesh's buffers (swapped with
-  // mc_verts / mc_faces after a clean) and the totals read back once per clean; all grow only
+  // small-part cleaning of the resident mesh (mesh_clean.cu): scratch arena and the totals read back once per clean; both
+  // grow only
   disn::DevBuffer cl_arena;
-  disn::DevBuffer cl_verts, cl_faces;
   disn::PinnedBuffer cl_totals_host;
   // signed distance field of the resident mesh (mesh_sdf.cu): scratch arena (BVH, edge bits, union-find parents, the
   // distance grid of host-output calls), pinned staging (mesh statistics, axis tables) and the phase timing events
@@ -359,15 +410,12 @@ int launch_cam_heads(disn_ctx* c, int B, const float* d_emb, const float* d_K, f
 // chamfer.cu
 int nn_distance(disn_ctx* c, const float* d_xyz1, int n, const float* d_xyz2, int m, int B, float* d_dist1,
                 int* d_idx1, float* d_dist2, int* d_idx2);
-// mc.cu
-int mc_run(disn_ctx* c, const float* d_sdf, int R, const double* bbox, float iso, int64_t* n_verts, int64_t* n_faces);
-int mc_fetch(disn_ctx* c, float* verts, int32_t* faces);
-// grow-only vertex [nv,3] and face [nf,3] arrays of a mesh, with 25 % + 1024 elements of slack
-int ensure_mesh(DevBuffer& verts, DevBuffer& faces, int64_t nv, int64_t nf);
+// mc.cu: the mesh of d_sdf [R,R,R] (3 R^3 < 2^32) becomes the resident mesh
+int mc_run(disn_ctx* c, const float* d_sdf, int R, const double* bbox, float iso);
 // in-place exclusive scan of d[0..n) on c->stream, total -> *d_total (device); `sums` = scan_scratch_elems(n) words
 int64_t scan_scratch_elems(int64_t n);
 int exclusive_scan(disn_ctx* c, uint32_t* d, int64_t n, uint32_t* d_total, uint32_t* sums);
-// mesh_clean.cu
+// mesh_clean.cu: uploads a host mesh whose arguments disn_mesh_load accepted
 int mesh_load(disn_ctx* c, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces);
 int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
                int64_t* n_kept, int64_t* n_verts, int64_t* n_faces);
@@ -399,10 +447,9 @@ int eval_grid_points(disn_ctx* c, int image, int R, const float* d_tm, const Ind
 int adaptive_run(disn_ctx* c, const float* field, int image, const float* d_tm, int32_t res, const double* sdf_params,
                  float iso, double band, int64_t* level_counts, int32_t* n_levels);
 // adaptive_mesh.cu: the mesh of adaptive_run's grid followed by mc_run, built from the surface blocks alone (s0 >= 2);
-// field / image / d_tm as for adaptive_run.  The mesh becomes the resident mesh (c->mc_verts / c->mc_faces).
+// field / image / d_tm as for adaptive_run.  The mesh becomes the resident mesh (c->mesh).
 int adaptive_mesh_run(disn_ctx* c, const float* field, int image, const float* d_tm, int32_t res, const double* sdf_params,
-                      float iso, double band, int64_t* level_counts, int32_t* n_levels, int64_t* n_verts,
-                      int64_t* n_faces);
+                      float iso, double band, int64_t* level_counts, int32_t* n_levels);
 // api.cu: the end of a call that builds the resident mesh from rc: empties the mesh on failure, reports its counts
 int finish_mesh_call(disn_ctx* c, int rc, int64_t* n_verts, int64_t* n_faces);
 // bytes held by the buffers of adaptive_mesh_run

@@ -11,7 +11,6 @@
 // Integer and atomic work bound by HBM / L2 latency; no tensor-core work.  Built with --fmad=false.
 #include <algorithm>
 #include <cstring>
-#include <utility>
 
 #include "common.cuh"
 
@@ -244,23 +243,17 @@ size_t carve(char* base, int64_t nv, int64_t nf, CleanBufs& b) {
 
 }  // namespace
 
-// Upload a host mesh into the resident mesh slot marching cubes fills (verts [nv,3] float32, faces [nf,3] int32 0-based).
+// Upload a host mesh into the resident mesh (verts [nv,3] float32, faces [nf,3] int32 0-based).
 int mesh_load(disn_ctx* c, const float* verts, int64_t nv, const int32_t* faces, int64_t nf) {
-  DISN_REQUIRE(nv >= 0 && nf >= 0 && (verts || nv == 0) && (faces || nf == 0), "bad mesh_load arguments");
-  DISN_REQUIRE(nv < ((int64_t)1 << 31) && 3 * nf < ((int64_t)1 << 31), "mesh too large for 32-bit indices");
-  for (int64_t i = 0; i < 3 * nf; ++i)
-    if (faces[i] < 0 || faces[i] >= nv)
-      DISN_REQUIRE(false, "face " + std::to_string(i / 3) + " references vertex " + std::to_string(faces[i]) +
-                              " outside [0, " + std::to_string(nv) + ")");
-  if (ensure_mesh(c->mc_verts, c->mc_faces, nv, nf)) return -1;
+  if (c->mesh.replace(nv, nf)) return -1;
   if (nv)
-    DISN_CUDA_OK(cudaMemcpyAsync(c->mc_verts.as<float>(), verts, (size_t)nv * 3 * sizeof(float), cudaMemcpyHostToDevice,
+    DISN_CUDA_OK(cudaMemcpyAsync(c->mesh.verts(), verts, (size_t)nv * 3 * sizeof(float), cudaMemcpyHostToDevice,
                                  c->stream));
   if (nf)
-    DISN_CUDA_OK(cudaMemcpyAsync(c->mc_faces.as<int32_t>(), faces, (size_t)nf * 3 * sizeof(int32_t),
-                                 cudaMemcpyHostToDevice, c->stream));
+    DISN_CUDA_OK(cudaMemcpyAsync(c->mesh.faces(), faces, (size_t)nf * 3 * sizeof(int32_t), cudaMemcpyHostToDevice,
+                                 c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
-  c->mc_nv = nv; c->mc_nf = nf;
+  c->mesh.commit(nv, nf);
   return 0;
 }
 
@@ -271,29 +264,29 @@ int mesh_load(disn_ctx* c, const float* verts, int64_t nv, const int32_t* faces,
 // int64 range guard is refused after that synchronisation and stays resident unchanged.
 int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face_component, int64_t* n_components,
                int64_t* n_kept, int64_t* n_verts, int64_t* n_faces) {
-  const int64_t nv = c->mc_nv, nf = c->mc_nf;
+  const int64_t nv = c->mesh.nv(), nf = c->mesh.nf();
   DISN_REQUIRE(nv < ((int64_t)1 << 31) && 3 * nf < ((int64_t)1 << 31), "mesh too large for 32-bit indices");
   auto out = [&](int64_t comps, int64_t kept) {
     if (n_components) *n_components = comps;
     if (n_kept) *n_kept = kept;
-    if (n_verts) *n_verts = c->mc_nv;
-    if (n_faces) *n_faces = c->mc_nf;
+    if (n_verts) *n_verts = c->mesh.nv();
+    if (n_faces) *n_faces = c->mesh.nf();
   };
   if (nf == 0) {          // no faces: nothing references a vertex, the cleaned mesh is empty
-    c->mc_nv = 0;
+    c->mesh.clear();
     out(0, 0);
     return 0;
   }
   CleanBufs b;
   const size_t bytes = carve(nullptr, nv, nf, b);
   if (c->cl_arena.ensure(bytes, bytes / 4) || c->cl_totals_host.ensure(T_COUNT * sizeof(uint32_t)) ||
-      ensure_mesh(c->cl_verts, c->cl_faces, nv, nf))
+      c->mesh.reserve_spare(nv, nf))
     return -1;
   carve(c->cl_arena.as<char>(), nv, nf, b);
 
   cudaStream_t s = c->stream;
-  const float* verts = c->mc_verts.as<float>();
-  const int32_t* faces = c->mc_faces.as<int32_t>();
+  const float* verts = c->mesh.verts();
+  const int32_t* faces = c->mesh.faces();
   uint32_t* T = b.totals;
   DISN_CUDA_OK(cudaMemsetAsync(b.offs, 0, (size_t)(nv + 1) * sizeof(uint32_t), s));
   DISN_CUDA_OK(cudaMemsetAsync(b.vflag, 0, (size_t)(nv + 1) * sizeof(uint32_t), s));
@@ -321,8 +314,8 @@ int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face
   DISN_CUDA_OK(cudaGetLastError());
   if (exclusive_scan(c, b.fflag, nf + 1, T + T_NF_OUT, b.scan)) return -1;
   if (exclusive_scan(c, b.vflag, nv + 1, T + T_NV_OUT, b.scan)) return -1;
-  clean_compact_verts_kernel<<<grid_of(nv), CL_THREADS, 0, s>>>(verts, nv, b.vflag, c->cl_verts.as<float>());
-  clean_compact_faces_kernel<<<grid_of(nf), CL_THREADS, 0, s>>>(faces, nf, b.fflag, b.vflag, c->cl_faces.as<int32_t>());
+  clean_compact_verts_kernel<<<grid_of(nv), CL_THREADS, 0, s>>>(verts, nv, b.vflag, c->mesh.spare_verts());
+  clean_compact_faces_kernel<<<grid_of(nf), CL_THREADS, 0, s>>>(faces, nf, b.fflag, b.vflag, c->mesh.spare_faces());
   c->launches += 2;
   DISN_CUDA_OK(cudaGetLastError());
   if (face_component)
@@ -337,10 +330,7 @@ int mesh_clean(disn_ctx* c, double dist_thresh, double num_thresh, int32_t* face
   DISN_REQUIRE(maxabs * (double)nv < 1073741824.0,
                "mesh_clean: max |coordinate| * n_verts = " + std::to_string(maxabs * (double)nv) +
                    " must stay below 2^30 (int64 fixed-point centroid sums)");
-  std::swap(c->mc_verts, c->cl_verts);
-  std::swap(c->mc_faces, c->cl_faces);
-  c->mc_nv = h[T_NV_OUT];
-  c->mc_nf = h[T_NF_OUT];
+  c->mesh.swap_spare(h[T_NV_OUT], h[T_NF_OUT]);
   out(h[T_NCOMP], h[T_NKEPT]);
   return 0;
 }

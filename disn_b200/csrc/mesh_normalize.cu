@@ -176,7 +176,7 @@ size_t carve(char* base, int64_t nf, int P, int64_t N, size_t cub_bytes, NormBuf
 // Shared by both entry points: checks, the area scan in part order and the part totals (on the device in b.part_q).
 // Host outputs: the statistics words after the first synchronisation and the shift s.
 int part_scan(disn_ctx* c, const int32_t* part_ids, int32_t P, int64_t N, NormBufs& b, int* shift) {
-  const int64_t nv = c->mc_nv, nf = c->mc_nf;
+  const int64_t nv = c->mesh.nv(), nf = c->mesh.nf();
   DISN_REQUIRE(nf > 0, "mesh_normalize: no resident mesh with faces (disn_mesh_load / disn_mc_run first)");
   DISN_REQUIRE(nv < ((int64_t)1 << 31) && 3 * nf < ((int64_t)1 << 31), "mesh too large for 32-bit indices");
   DISN_REQUIRE(P >= 1 && P <= nf && (part_ids || P == 1),
@@ -204,8 +204,8 @@ int part_scan(disn_ctx* c, const int32_t* part_ids, int32_t P, int64_t N, NormBu
   if (c->nm_arena.ensure(bytes, bytes / 4) || c->nm_host.ensure(W_COUNT * sizeof(unsigned long long))) return -1;
   carve(c->nm_arena.as<char>(), nf, P, N, cub_bytes, b);
   cudaStream_t s = c->stream;
-  const float* verts = c->mc_verts.as<float>();
-  const int32_t* faces = c->mc_faces.as<int32_t>();
+  const float* verts = c->mesh.verts();
+  const int32_t* faces = c->mesh.faces();
   const int32_t* d_order = part_ids ? b.order : nullptr;
   if (part_ids)
     DISN_CUDA_OK(cudaMemcpyAsync(b.order, order.data(), (size_t)nf * sizeof(int32_t), cudaMemcpyHostToDevice, s));
@@ -251,10 +251,10 @@ int mesh_part_areas(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, int64
 int mesh_normalize(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, const int64_t* amounts, const double* draws,
                    int64_t n_draws, const double* given, double* centroid_out, double* m_out, double* samples_out) {
   cudaStream_t s = c->stream;
-  const int64_t nv = c->mc_nv;
+  const int64_t nv = c->mesh.nv();
   double cen[3], m;
   if (given) {
-    DISN_REQUIRE(c->mc_nf > 0, "mesh_normalize: no resident mesh with faces (disn_mesh_load / disn_mc_run first)");
+    DISN_REQUIRE(c->mesh.nf() > 0, "mesh_normalize: no resident mesh with faces (disn_mesh_load / disn_mc_run first)");
     for (int a = 0; a < 3; ++a) cen[a] = given[a];
     m = given[3];
     DISN_REQUIRE(std::isfinite(cen[0]) && std::isfinite(cen[1]) && std::isfinite(cen[2]) && std::isfinite(m) && m > 0.0,
@@ -262,7 +262,7 @@ int mesh_normalize(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, const 
     if (c->nm_arena.ensure(W_COUNT * sizeof(unsigned long long)) || c->nm_host.ensure(sizeof(unsigned long long))) return -1;
     unsigned long long* st = c->nm_arena.as<unsigned long long>();
     DISN_CUDA_OK(cudaMemsetAsync(st, 0, sizeof(unsigned long long), s));
-    nm_check_kernel<<<grid_of(3 * nv), NM_THREADS, 0, s>>>(c->mc_verts.as<float>(), nv, st);
+    nm_check_kernel<<<grid_of(3 * nv), NM_THREADS, 0, s>>>(c->mesh.verts(), nv, st);
     c->launches++;
     DISN_CUDA_OK(cudaGetLastError());
     unsigned long long* hs = c->nm_host.as<unsigned long long>();
@@ -272,8 +272,8 @@ int mesh_normalize(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, const 
   } else {
     DISN_REQUIRE(amounts && (draws || n_draws == 0) && n_draws >= 0, "mesh_normalize: amounts and draws are required");
     // host-only checks of the caller's arrays first: nothing is sized from them before they agree
-    DISN_REQUIRE(c->mc_nf > 0, "mesh_normalize: no resident mesh with faces (disn_mesh_load / disn_mc_run first)");
-    DISN_REQUIRE(n_parts >= 1 && n_parts <= c->mc_nf && (part_ids || n_parts == 1),
+    DISN_REQUIRE(c->mesh.nf() > 0, "mesh_normalize: no resident mesh with faces (disn_mesh_load / disn_mc_run first)");
+    DISN_REQUIRE(n_parts >= 1 && n_parts <= c->mesh.nf() && (part_ids || n_parts == 1),
                  "mesh_normalize: 1 <= n_parts <= n_faces (part_ids may be NULL only for one part)");
     std::vector<long long> pq(n_parts), sstart(n_parts + 1, 0);
     for (int p = 0; p < n_parts; ++p) {
@@ -298,7 +298,7 @@ int mesh_normalize(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, const 
     DISN_CUDA_OK(cudaMemcpyAsync(b.sample_start, sstart.data(), (size_t)(n_parts + 1) * sizeof(long long),
                                  cudaMemcpyHostToDevice, s));
     DISN_CUDA_OK(cudaMemcpyAsync(b.draws, draws, (size_t)N * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
-    nm_sample_kernel<<<grid_of(N), NM_THREADS, 0, s>>>(c->mc_verts.as<float>(), c->mc_faces.as<int32_t>(),
+    nm_sample_kernel<<<grid_of(N), NM_THREADS, 0, s>>>(c->mesh.verts(), c->mesh.faces(),
                                                        part_ids ? b.order : nullptr, b.incl, b.part_start,
                                                        b.sample_start, b.part_q, n_parts, b.draws, N, b.samples,
                                                        b.stats);
@@ -319,7 +319,7 @@ int mesh_normalize(disn_ctx* c, const int32_t* part_ids, int32_t n_parts, const 
     for (int a = 0; a < 3; ++a) cen[a] = ((double)(long long)hs[W_SUM + a] / (double)N) * 0x1p-32;
     DISN_REQUIRE(m > 0.0 && std::isfinite(m), "mesh_normalize: every sample lies on the centroid (m = 0)");
   }
-  nm_transform_kernel<<<grid_of(3 * nv), NM_THREADS, 0, s>>>(c->mc_verts.as<float>(), nv, cen[0], cen[1], cen[2], m);
+  nm_transform_kernel<<<grid_of(3 * nv), NM_THREADS, 0, s>>>(c->mesh.verts(), nv, cen[0], cen[1], cen[2], m);
   c->launches++;
   DISN_CUDA_OK(cudaGetLastError());
   DISN_CUDA_OK(cudaStreamSynchronize(s));

@@ -467,7 +467,7 @@ size_t carve(char* base, int64_t nf, int64_t nleaf_slots, int R, bool own_dist, 
 // boundary flags -> sign; a second synchronisation at the end (output copy, the raster work total).
 int mesh_sdf(disn_ctx* c, int32_t res, const double* bbox, double expand_rate, double sigma, float* out,
              double* bbox_out, bool device_out) {
-  const int64_t nv = c->mc_nv, nf = c->mc_nf;
+  const int64_t nv = c->mesh.nv(), nf = c->mesh.nf();
   DISN_REQUIRE(nf > 0, "mesh_sdf: no resident mesh with faces (disn_mesh_load / disn_mc_run first)");
   DISN_REQUIRE(nv < ((int64_t)1 << 31) && 3 * nf < ((int64_t)1 << 31), "mesh too large for 32-bit indices");
   const int R = res + 1;
@@ -495,8 +495,8 @@ int mesh_sdf(disn_ctx* c, int32_t res, const double* bbox, double expand_rate, d
   if (c->sdf_arena.ensure(bytes, bytes / 4)) return -1;
   carve(c->sdf_arena.as<char>(), nf, nleaf_slots, R, !device_out, cub_bytes, b);
   float* dist = device_out ? out : b.dist;
-  const float* verts = c->mc_verts.as<float>();
-  const int32_t* faces = c->mc_faces.as<int32_t>();
+  const float* verts = c->mesh.verts();
+  const int32_t* faces = c->mesh.faces();
 
   // statistics: AABB (ordered ints, min words start at all-ones) and the non-finite flag
   DISN_CUDA_OK(cudaEventRecord(c->sdf_ev[0], s));

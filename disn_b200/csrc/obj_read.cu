@@ -322,12 +322,11 @@ int obj_token_to_float(const char* s, int64_t len, float* out, bool* overflow) {
   return 0;
 }
 
-// Reads `path` into the resident mesh (c->mc_verts / c->mc_faces); see the file comment.  On success the context is in
-// the state disn_mesh_load(read_obj(path)) leaves; on any failure the resident mesh is empty.
+// Reads `path` into the resident mesh (c->mesh); see the file comment.  On success the context is in the state
+// disn_mesh_load(read_obj(path)) leaves; on any failure disn_obj_read empties the resident mesh.
 int obj_read(disn_ctx* c, const char* path, bool parts, int64_t* n_parts) {
   const std::string spath(path);
   auto refuse = [&](const std::string& msg) { set_error(msg); return DISN_ERR_OBJ_UNSUPPORTED; };
-  c->mc_nv = c->mc_nf = 0;                                   // the resident mesh is replaced from here on
   c->obj_host_tokens = 0;
   c->obj_overflows = 0;
   c->obj_parts_ready = false;
@@ -425,11 +424,11 @@ int obj_read(disn_ctx* c, const char* path, bool parts, int64_t* n_parts) {
   const size_t bytes2 = carve_lists(nullptr, slow_cap, nf, parts, o);
   if (c->obj_lists.ensure(bytes2, bytes2 / 4)) return -1;
   carve_lists(c->obj_lists.as<char>(), slow_cap, nf, parts, o);
-  if (ensure_mesh(c->mc_verts, c->mc_faces, nv, nf)) return -1;
+  if (c->mesh.replace(nv, nf)) return -1;
   const unsigned long long init2[2] = {kNoStatus, 0ull};
   DISN_CUDA_OK(cudaMemcpyAsync(o.counters, init2, sizeof(init2), cudaMemcpyHostToDevice, s));
   if (nv + nf) {
-    ParseArgs a{db, n, o.starts, nl, o.type, o.vf, o.mtl, nv, c->mc_verts.as<float>(), c->mc_faces.as<int32_t>(),
+    ParseArgs a{db, n, o.starts, nl, o.type, o.vf, o.mtl, nv, c->mesh.verts(), c->mesh.faces(),
                 o.face_mtl, o.slow_off, o.slow_dst, o.counters};
     obj_parse_kernel<<<blocks_for(nl), OBJ_THREADS, 0, s>>>(a);
     c->launches++;
@@ -472,7 +471,7 @@ int obj_read(disn_ctx* c, const char* path, bool parts, int64_t* n_parts) {
       overflow |= of;
     }
     DISN_CUDA_OK(cudaMemcpyAsync(o.slow_val, hval, ns * sizeof(float), cudaMemcpyHostToDevice, s));
-    obj_patch_kernel<<<blocks_for(ns), OBJ_THREADS, 0, s>>>(c->mc_verts.as<float>(), o.slow_dst, o.slow_val, ns);
+    obj_patch_kernel<<<blocks_for(ns), OBJ_THREADS, 0, s>>>(c->mesh.verts(), o.slow_dst, o.slow_val, ns);
     c->launches++;
     DISN_CUDA_OK(cudaGetLastError());
   }
@@ -523,8 +522,7 @@ int obj_read(disn_ctx* c, const char* path, bool parts, int64_t* n_parts) {
   DISN_CUDA_OK(cudaStreamSynchronize(s));
   c->obj_phase_ms[4] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
   for (int k = 0; k < 4; ++k) DISN_CUDA_OK(cudaEventElapsedTime(&c->obj_phase_ms[k], c->obj_ev[k], c->obj_ev[k + 1]));
-  c->mc_nv = nv;
-  c->mc_nf = nf;
+  c->mesh.commit(nv, nf);
   if (n_parts) *n_parts = np;
   return 0;
 }

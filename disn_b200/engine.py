@@ -53,8 +53,6 @@ class Engine:
         self._h = C.c_void_p()
         check(self.lib.disn_create(C.byref(cfg), C.byref(self._h)))
         self.batch = 0
-        self._mesh_faces = 0        # face count of the resident mesh (sizes clean_mesh's labels)
-        self._mesh_verts = 0        # vertex count of the resident mesh (sizes fetch_mesh)
         self.last_clean = None
         self.obj_fallbacks = 0      # files read_obj handed to the Python reader
 
@@ -327,7 +325,8 @@ class Engine:
     def marching_cubes(self, sdf, bbox, iso: float = 0.0, device_ptr: int | None = None, R: int | None = None,
                        fetch: bool = True):
         """sdf [R,R,R] (z,y,x) host array, or a device pointer -> (verts [V,3] float32, faces [F,3] int32 0-based).
-        The welded mesh also stays in HBM (write_mesh_obj); fetch=False returns only the counts."""
+        The welded mesh also stays in HBM as the resident mesh (write_mesh_obj, clean_mesh); fetch=False returns only
+        the counts.  A failed call leaves the resident mesh empty."""
         bb = (C.c_double * 6)(*[float(v) for v in bbox])
         if device_ptr is None:
             a = _f32(sdf)
@@ -338,38 +337,31 @@ class Engine:
             ptr, flags = C.c_void_p(device_ptr), DISN_DEVICE_PTR
         nv, nf = C.c_int64(0), C.c_int64(0)
         check(self.lib.disn_mc_run(self._h, ptr, R, bb, float(iso), flags, C.byref(nv), C.byref(nf)))
-        self._mesh_faces = nf.value
-        self._mesh_verts = nv.value
         if not fetch:
             return nv.value, nf.value
-        verts = np.empty((nv.value, 3), dtype=np.float32)
-        faces = np.empty((nf.value, 3), dtype=np.int32)
-        if nv.value and nf.value:
-            check(self.lib.disn_mc_fetch(self._h, verts.ctypes.data_as(C.c_void_p), faces.ctypes.data_as(C.c_void_p)))
-        return verts, faces
+        return self._fetch(nv.value, nf.value)
 
     def write_mesh_obj(self, path: str):
-        """OBJ of the mesh left in HBM by the last marching_cubes / load_mesh / clean_mesh call (reference mesher's output
-        conventions)."""
+        """OBJ of the resident mesh, as the last marching_cubes / load_mesh / clean_mesh call left it (reference mesher's
+        output conventions)."""
         check(self.lib.disn_mc_write_obj(self._h, path.encode()))
 
     def load_mesh(self, verts, faces):
-        """Upload a mesh (verts [V,3] float32, faces [F,3] 0-based) into the resident slot marching_cubes fills."""
+        """Upload a mesh (verts [V,3] float32, faces [F,3] 0-based) into the resident slot marching_cubes fills.  A face
+        index outside [0, V) is refused and leaves the resident mesh as it was."""
         v = _f32(verts).reshape(-1, 3)
         f = np.ascontiguousarray(faces, np.int32).reshape(-1, 3)
         check(self.lib.disn_mesh_load(self._h, v.ctypes.data_as(C.c_void_p), len(v), f.ctypes.data_as(C.c_void_p), len(f)))
-        self._mesh_faces = len(f)
-        self._mesh_verts = len(v)
 
     def read_obj(self, path, parts: bool = False, load: bool = False):
         """create_sdf.read_obj(path), or read_obj_parts(path) with parts=True, parsed on the device (disn_obj_read): the
         same arrays bit for bit, and the same names.  The mesh stays resident, as after load_mesh.  A file outside the
         device reader's grammar (or one it finds invalid, or cannot open) is read by the Python reader instead, which
-        raises what it raises; `obj_fallbacks` counts those files, and load=True then uploads what it returned."""
+        raises what it raises; `obj_fallbacks` counts those files, and load=True then uploads what it returned (the
+        resident mesh is empty otherwise)."""
         nv, nf, npart = C.c_int64(0), C.c_int64(0), C.c_int32(0)
         rc = self.lib.disn_obj_read(self._h, os.fsencode(path), _lib.DISN_OBJ_PARTS if parts else 0, C.byref(nv),
                                     C.byref(nf), C.byref(npart))
-        self._mesh_verts, self._mesh_faces = nv.value, nf.value
         if rc == _lib.DISN_ERR_OBJ_UNSUPPORTED:
             from .create_sdf import read_obj, read_obj_parts
             self.obj_fallbacks += 1
@@ -382,7 +374,7 @@ class Engine:
         check(self.lib.disn_obj_read_stats(self._h, counts.ctypes.data_as(C.c_void_p), None))
         if counts[1]:       # a finite coordinate overflowed float32: numpy's own warning, as the cast in read_obj gives
             np.array([np.finfo(np.float64).max]).astype(np.float32)
-        verts, faces = self.fetch_mesh()
+        verts, faces = self._fetch(nv.value, nf.value)
         if not parts:
             return verts, faces
         pid = np.empty(nf.value, np.int32)
@@ -405,33 +397,40 @@ class Engine:
         return {"host_tokens": int(counts[0]), "overflows": int(counts[1]),
                 "phase_ms": dict(zip(("upload", "lines", "classify", "parse", "host"), list(ms)))}
 
+    def mesh_counts(self):
+        """(n_verts, n_faces) of the resident mesh, read from the library's host-side state (no device work)."""
+        nv, nf = C.c_int64(0), C.c_int64(0)
+        check(self.lib.disn_mesh_counts(self._h, C.byref(nv), C.byref(nf)))
+        return nv.value, nf.value
+
     def fetch_mesh(self):
-        """The resident mesh (last marching_cubes / load_mesh / clean_mesh / normalize_mesh) -> (verts, faces)."""
-        verts = np.empty((self._mesh_verts, 3), dtype=np.float32)
-        faces = np.empty((self._mesh_faces, 3), dtype=np.int32)
-        if len(verts) or len(faces):        # the library copies each array only when the resident mesh has entries
+        """The resident mesh (last marching_cubes / load_mesh / read_obj / mesh_grid_adaptive / clean_mesh /
+        normalize_mesh, or a C-ABI call that wrote it) -> (verts, faces), sized by mesh_counts()."""
+        return self._fetch(*self.mesh_counts())
+
+    def _fetch(self, nv: int, nf: int):
+        """The resident mesh, whose counts are nv / nf -> (verts [nv,3] float32, faces [nf,3] int32)."""
+        verts = np.empty((nv, 3), dtype=np.float32)
+        faces = np.empty((nf, 3), dtype=np.int32)
+        if nv or nf:        # the library copies each array only when the resident mesh has entries
             check(self.lib.disn_mc_fetch(self._h, verts.ctypes.data_as(C.c_void_p), faces.ctypes.data_as(C.c_void_p)))
         return verts, faces
 
     def clean_mesh(self, dist_thresh: float = 0.5, num_thresh: float = 0.3, fetch: bool = True, want_labels: bool = False):
         """postprocessing/clean_smallparts.py:38-54 on the resident mesh, in place: drop every edge-connected component
         with n_c <= max n_c * num_thresh vertices or a centroid at distance >= dist_thresh from the origin.
-        -> (verts, faces), plus the per-face component labels of the input mesh if want_labels; fetch=False returns
-        the MeshCleanCounts instead of the mesh (and the labels).  The counts of the last call are in `last_clean`."""
-        labels = np.empty(self._mesh_faces, np.int32) if want_labels else None
+        -> (verts, faces), plus the per-face component labels of the input mesh (sized by mesh_counts()) if
+        want_labels; fetch=False returns the MeshCleanCounts instead of the mesh (and the labels).  The counts of the
+        last call are in `last_clean`."""
+        labels = np.empty(self.mesh_counts()[1], np.int32) if want_labels else None
         nc, nk, nv, nf = (C.c_int64(0) for _ in range(4))
         check(self.lib.disn_mesh_clean(self._h, float(dist_thresh), float(num_thresh),
                                        None if labels is None else labels.ctypes.data_as(C.c_void_p),
                                        C.byref(nc), C.byref(nk), C.byref(nv), C.byref(nf)))
-        self._mesh_faces = nf.value
-        self._mesh_verts = nv.value
         self.last_clean = MeshCleanCounts(nv.value, nf.value, nc.value, nk.value)
         if not fetch:
             return (self.last_clean, labels) if want_labels else self.last_clean
-        verts = np.empty((nv.value, 3), dtype=np.float32)
-        faces = np.empty((nf.value, 3), dtype=np.int32)
-        if nv.value and nf.value:
-            check(self.lib.disn_mc_fetch(self._h, verts.ctypes.data_as(C.c_void_p), faces.ctypes.data_as(C.c_void_p)))
+        verts, faces = self._fetch(nv.value, nf.value)
         return (verts, faces, labels) if want_labels else (verts, faces)
 
     def mesh_sdf(self, res: int, bbox=None, expand_rate: float = 1.2, sigma: float = 0.0, verts=None, faces=None,
@@ -610,26 +609,20 @@ class Engine:
         """Coarse-to-fine mesh of encoded image `image` without a dense grid (DESIGN.md §4.10): bit for bit the mesh
         marching_cubes makes of eval_grid_adaptive's grid, with memory proportional to the evaluated points; sdf_res up to
         2048.  The mesh stays resident (clean_mesh, write_mesh_obj) -> (verts, faces, level_counts), or with fetch=False
-        ((n_verts, n_faces), level_counts)."""
+        ((n_verts, n_faces), level_counts).  A call that fails after its arguments are accepted leaves the resident mesh
+        empty."""
         sp = np.ascontiguousarray(sdf_params, dtype=np.float64).reshape(6)
         t = _f32(trans_mat).reshape(4, 3)
         counts = np.zeros(5, np.int64)
         nl = C.c_int32(0)
-        # the library reports the resident counts whenever it may have changed the mesh, also when the call fails (the
-        # mesh is then empty); an argument error leaves both, so start from the counts of the mesh held now
-        nv, nf = C.c_int64(self._mesh_verts), C.c_int64(self._mesh_faces)
-        rc = self.lib.disn_mesh_grid_adaptive(self._h, sp.ctypes.data_as(C.POINTER(C.c_double)), t.ctypes.data_as(C.c_void_p),
-                                              image, sdf_res, float(iso), float(band), counts.ctypes.data_as(C.c_void_p),
-                                              C.byref(nl), C.byref(nv), C.byref(nf))
-        self._mesh_verts, self._mesh_faces = nv.value, nf.value
-        check(rc)
+        nv, nf = C.c_int64(0), C.c_int64(0)
+        check(self.lib.disn_mesh_grid_adaptive(self._h, sp.ctypes.data_as(C.POINTER(C.c_double)),
+                                               t.ctypes.data_as(C.c_void_p), image, sdf_res, float(iso), float(band),
+                                               counts.ctypes.data_as(C.c_void_p), C.byref(nl), C.byref(nv), C.byref(nf)))
         levels = [int(v) for v in counts[:nl.value]]
         if not fetch:
             return (nv.value, nf.value), levels
-        verts = np.empty((nv.value, 3), dtype=np.float32)
-        faces = np.empty((nf.value, 3), dtype=np.int32)
-        if nv.value and nf.value:
-            check(self.lib.disn_mc_fetch(self._h, verts.ctypes.data_as(C.c_void_p), faces.ctypes.data_as(C.c_void_p)))
+        verts, faces = self._fetch(nv.value, nf.value)
         return verts, faces, levels
 
     def fetch(self, dev_ptr: int, shape, dtype=np.float32) -> np.ndarray:

@@ -138,9 +138,12 @@ int disn_marching_cubes(disn_ctx* ctx, const float* sdf, int32_t R, const double
 /* Device-resident variant of the driver's tail (test/create_sdf.py:277-323 without the .dist round trip through the
  * file system): disn_eval_grid_resident leaves the whole [B,R,R,R] grid (pred/sdf_weight) in HBM and returns its device
  * address (valid until the next call on this context); disn_mc_run meshes one [R,R,R] field (device pointer with
- * DISN_DEVICE_PTR, e.g. grid + b*R^3, or a host array) and keeps the welded mesh in HBM; disn_mc_fetch copies it to host
- * buffers of n_verts*3 floats / n_faces*3 int32; disn_mc_write_obj writes it in disn_write_obj's format; disn_fetch is
- * a synchronous device->host copy on the context's stream (e.g. to keep the .dist artefact). */
+ * DISN_DEVICE_PTR, e.g. grid + b*R^3, or a host array; 2 <= R and 3 R^3 < 2^32) and keeps the welded mesh in HBM as the
+ * resident mesh.  Once its arguments are accepted, *n_verts / *n_faces (each may be NULL) receive the resident mesh's
+ * counts, also on failure: a failed call (out of memory, a CUDA error) leaves the resident mesh empty.  disn_mc_fetch
+ * copies the resident mesh to host buffers of n_verts*3 floats / n_faces*3 int32; disn_mesh_counts reports its counts
+ * from host-side state (no device work, no synchronisation); disn_mc_write_obj writes it in disn_write_obj's format;
+ * disn_fetch is a synchronous device->host copy on the context's stream (e.g. to keep the .dist artefact). */
 int disn_eval_grid_resident(disn_ctx* ctx, const double* sdf_params, const float* trans_mat, int32_t B,
                             int32_t sdf_res, float** out_dev);
 
@@ -179,13 +182,15 @@ int disn_mesh_grid_adaptive(disn_ctx* ctx, const double* sdf_params, const float
 int disn_mc_run(disn_ctx* ctx, const float* sdf, int32_t R, const double* bbox, float iso, uint32_t flags,
                 int64_t* n_verts, int64_t* n_faces);
 int disn_mc_fetch(disn_ctx* ctx, float* verts, int32_t* faces);
+int disn_mesh_counts(disn_ctx* ctx, int64_t* n_verts, int64_t* n_faces);
 int disn_mc_write_obj(disn_ctx* ctx, const char* path);
 int disn_fetch(disn_ctx* ctx, const void* dev, void* host, int64_t bytes);
 
 /* Small-part removal, the reference's clean_single_mesh (postprocessing/clean_smallparts.py:38-54), on the resident mesh
  * of disn_mc_run / disn_mesh_load; disn_mc_fetch and disn_mc_write_obj then return the cleaned mesh.
  *   disn_mesh_load: uploads a host mesh (verts [n_verts,3] float32, faces [n_faces,3] int32 0-based) into that slot; a
- *     face index outside [0, n_verts) is an error.
+ *     face index outside [0, n_verts) is an error and leaves the resident mesh as it was.  Once the arguments are
+ *     accepted, a failed call (out of memory, a CUDA error) leaves the resident mesh empty.
  *   disn_mesh_clean: components = faces connected through shared undirected edges {a,b}, a != b (PyMesh "face"
  *     connectivity), numbered in order of their smallest face; n_c = distinct vertices of component c; centroid from
  *     fixed-point sums (round(v * 2^32) in int64); keep c iff n_c > max n_c * num_thresh and |centroid| < dist_thresh

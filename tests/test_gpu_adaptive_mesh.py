@@ -39,13 +39,11 @@ def dense_from_field(eng, F, res, box, iso, band):
 def mesh_from_field(eng, F, res, box, iso, band):
     counts = np.zeros(5, np.int64)
     nl = C.c_int32(0)
-    nv, nf = C.c_int64(eng._mesh_verts), C.c_int64(eng._mesh_faces)
-    try:
-        from_field(eng, "disn_mesh_adaptive_from_field", F, res, box, iso, band, counts.ctypes.data_as(C.c_void_p),
-                   C.byref(nl), C.byref(nv), C.byref(nf))
-    finally:
-        eng._mesh_verts, eng._mesh_faces = nv.value, nf.value
-    v, f = eng.fetch_mesh()
+    nv, nf = C.c_int64(-1), C.c_int64(-1)
+    from_field(eng, "disn_mesh_adaptive_from_field", F, res, box, iso, band, counts.ctypes.data_as(C.c_void_p),
+               C.byref(nl), C.byref(nv), C.byref(nf))
+    v, f = eng.fetch_mesh()         # sized from the library's counts, which the raw call above set
+    assert (len(v), len(f)) == (nv.value, nf.value)
     return v, f, [int(c) for c in counts[:nl.value]]
 
 
@@ -59,7 +57,8 @@ def same(a, b):
 @pytest.mark.parametrize("res,kind,band", [(64, "noise", 0.5), (64, "smooth", 0.0), (64, "smooth", np.inf),
                                            (128, "noise", 1.0), (128, "smooth", 2.0), (256, "smooth", 1.0),
                                            (512, "smooth", 1.0), (96, "ties", 0.0), (96, "subnormal", 0.0)])
-def test_from_field_equals_dense_path(engines, res, kind, band):
+def test_from_field_fetched_mesh_equals_dense_path(engines, res, kind, band):
+    """the mesh a raw disn_mesh_adaptive_from_field call leaves resident, as fetch_mesh returns it"""
     eng = engines("fp32")
     R = res + 1
     F = make_field(kind, BOX, R, seed=res)
@@ -75,7 +74,8 @@ def test_from_field_equals_dense_path(engines, res, kind, band):
         same(got, twin)
 
 
-def test_exact_distance_field(engines):
+def test_exact_distance_field_fetched_mesh_equals_dense_path(engines):
+    """as above on the exact distance field of a torus"""
     eng = engines("fp32")
     res, R = 256, 257
     v, f = analytic_mesh("torus", 15)
@@ -208,9 +208,10 @@ def test_errors_leave_context_usable(weights, engines, demo_img, tmp_path):
         diag("disn_mesh_adaptive_phase_ms", eng._h, ms.ctypes.data_as(C.c_void_p))
     with pytest.raises(DisnError, match="no coarse-to-fine mesh"):
         diag("disn_mesh_adaptive_edges", eng._h, 0, 1, np.zeros(1, np.int64).ctypes.data_as(C.c_void_p))
-    # f16f8 overflow is loud, empties the resident mesh in the library and in Python alike, and does not stick
+    # f16f8 overflow is loud, empties the resident mesh, and does not stick
     fresh = Engine(device=0, precision="f16f8")
     try:
+        assert fresh.mesh_counts() == (0, 0)
         fresh.load_weights(weights)
         fresh.encode(demo_img)
         small = fresh.mesh_grid_adaptive(BOX, tm, 16, iso=median_iso(fresh))
@@ -219,9 +220,10 @@ def test_errors_leave_context_usable(weights, engines, demo_img, tmp_path):
         fresh.encode(demo_img)
         with pytest.raises(DisnError, match="fp16 range"):
             fresh.mesh_grid_adaptive(BOX, tm, 128, iso=0.0)
+        assert fresh.mesh_counts() == (0, 0)
         v, f = fresh.fetch_mesh()
         assert v.shape == (0, 3) and f.shape == (0, 3)
-        fresh.write_mesh_obj(str(tmp_path / "after_overflow.obj"))      # the library's counts, not Python's
+        fresh.write_mesh_obj(str(tmp_path / "after_overflow.obj"))      # written from the library's counts
         with open(tmp_path / "after_overflow.obj") as fh:
             head = fh.read(4096)
         assert "Number of vertices: 0\n" in head and "Number of faces: 0\n" in head

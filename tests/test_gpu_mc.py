@@ -33,8 +33,23 @@ def test_marching_cubes_matches_oracle_bit_exact(engine, case):
     assert v.shape == rv.shape and f.shape == rf.shape
     np.testing.assert_array_equal(f, rf)            # integer topology: bit-exact
     np.testing.assert_array_equal(v, rv)            # same float64 formula, same roundings
+    assert engine.mesh_counts() == (len(rv), len(rf))
     if case.startswith("sphere"):
         assert mco.is_closed_manifold(f) and mco.signed_volume(v, f) > 0     # outward winding like demo/result.obj
+
+
+def test_refused_arguments_leave_the_resident_mesh(engine):
+    """disn_mc_run checks its arguments before it replaces the resident mesh (a grid whose vertex ids need more than 32
+    bits is refused before anything is read from it)."""
+    from disn_b200._lib import DisnError
+    v, f = engine.marching_cubes(_sphere(17), [-1, -1, -1, 1, 1, 1])
+    assert len(f) > 0
+    field = engine.field_buffer(2)
+    for R, what in ((1, "at least 2 samples"), (1128, "32-bit vertex ids")):
+        with pytest.raises(DisnError, match=what):
+            engine.marching_cubes(None, [-1, -1, -1, 1, 1, 1], device_ptr=field, R=R)
+        assert engine.mesh_counts() == (len(v), len(f))
+    np.testing.assert_array_equal(engine.fetch_mesh()[1], f)
 
 
 def test_mesh_of_predicted_grid_is_consistent(engine, he_weights):

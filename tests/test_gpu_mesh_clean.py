@@ -131,17 +131,21 @@ def test_empty_context_and_errors(tmp_path):
     try:
         v, f = eng.clean_mesh()                                # a fresh context holds the empty mesh
         assert v.shape == (0, 3) and f.shape == (0, 3) and eng.last_clean.n_components == 0
+        assert eng.mesh_counts() == (0, 0)
         tri = np.array([[0, 0, 0], [0.25, 0, 0], [0, 0.25, 0]], np.float32)
+        eng.load_mesh(tri, [[0, 1, 2], [0, 2, 1]])
         with pytest.raises(DisnError, match="outside"):
             eng.load_mesh(tri, [[0, 1, 3]])
         with pytest.raises(DisnError, match="outside"):
             eng.load_mesh(tri, [[0, -1, 2]])
+        assert eng.mesh_counts() == (3, 2)                    # a refused upload leaves the mesh loaded before
         eng.load_mesh(tri * np.float32(2 ** 29), [[0, 1, 2]])  # max|v| * n_verts = 3 * 2^27 ... below 2^30
         eng.clean_mesh()
         big = tri * np.float32(2 ** 31)                        # 2^29 * 3 >= 2^30
         eng.load_mesh(big, [[0, 1, 2]])
         with pytest.raises(DisnError, match="2\\^30"):
             eng.clean_mesh()
+        assert eng.mesh_counts() == (3, 1)                    # refused after the synchronisation: still resident
         nan = tri.copy()
         nan[1, 0] = np.nan
         eng.load_mesh(nan, [[0, 1, 2]])

@@ -237,7 +237,7 @@ def test_c_abi_refusals_name_path_and_line_and_empty_the_mesh(eng, tmp_path):
         assert rc == _lib.DISN_ERR_OBJ_UNSUPPORTED, (case, rc, msg)
         assert msg.startswith("%s:%d: " % (p, line)) and what in msg, (case, msg)
         assert (nv.value, nf.value) == (0, 0)
-        eng._mesh_verts = eng._mesh_faces = 0
+        assert eng.mesh_counts() == (0, 0)
         v, f = np.empty((0, 3), np.float32), np.empty((0, 3), np.int32)
         _lib.check(lib.disn_mc_fetch(eng._h, v.ctypes.data_as(C.c_void_p), f.ctypes.data_as(C.c_void_p)))
         clean = eng.clean_mesh(fetch=False)
