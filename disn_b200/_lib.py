@@ -45,6 +45,8 @@ EXPORTS = {
     "disn_write_dist": (C.c_int, [C.c_char_p, C.c_int32, C.POINTER(C.c_double), C.c_void_p]),
     "disn_cam_estimate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                     C.c_void_p, C.c_void_p]),
+    "disn_cam_metrics": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                   C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "disn_nn_distance": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "disn_write_obj": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]),

@@ -393,8 +393,6 @@ int disn_cam_estimate(disn_ctx* c, const float* imgs, int32_t B, int32_t H, int3
   DISN_REQUIRE(c && imgs && out_trans_mat, "null argument");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
   DISN_REQUIRE(B >= 1 && B <= c->cfg.max_batch, "batch exceeds max_batch of the context");
-  if (encoder_run(c, imgs, B, H, W, C, false, /*embedding_only=*/true)) return -1;
-  static const float kDefaultK[9] = {149.84375f, 0.f, 68.5f, 0.f, 149.84375f, 68.5f, 0.f, 0.f, 1.f};
   float *dK, *dRT, *dTM;
   auto carve = [&](char* base) {
     Arena a{base};
@@ -405,8 +403,7 @@ int disn_cam_estimate(disn_ctx* c, const float* imgs, int32_t B, int32_t H, int3
   };
   if (c->nn_scratch.ensure(carve(nullptr))) return -1;
   carve(c->nn_scratch.as<char>());
-  DISN_CUDA_OK(cudaMemcpyAsync(dK, K ? K : kDefaultK, 9 * 4, cudaMemcpyHostToDevice, c->stream));
-  if (launch_cam_heads(c, B, c->emb.as<float>(), dK, dRT, dTM)) return -1;
+  if (cam_predict(c, imgs, B, H, W, C, K, dK, dRT, dTM)) return -1;
   if (out_rt) DISN_CUDA_OK(cudaMemcpyAsync(out_rt, dRT, (size_t)B * 12 * 4, cudaMemcpyDeviceToHost, c->stream));
   DISN_CUDA_OK(cudaMemcpyAsync(out_trans_mat, dTM, (size_t)B * 12 * 4, cudaMemcpyDeviceToHost, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));

@@ -103,4 +103,119 @@ int launch_cam_heads(disn_ctx* c, int B, const float* d_emb, const float* d_K, f
   return 0;
 }
 
+int cam_predict(disn_ctx* c, const float* imgs, int B, int H, int W, int C, const float* K, float* d_K, float* d_rt,
+                float* d_tm) {
+  if (encoder_run(c, imgs, B, H, W, C, false, /*embedding_only=*/true)) return -1;
+  static const float kDefaultK[9] = {149.84375f, 0.f, 68.5f, 0.f, 149.84375f, 68.5f, 0.f, 0.f, 1.f};
+  DISN_CUDA_OK(cudaMemcpyAsync(d_K, K ? K : kDefaultK, 9 * 4, cudaMemcpyHostToDevice, c->stream));
+  return launch_cam_heads(c, B, c->emb.as<float>(), d_K, d_rt, d_tm);
+}
+
+namespace {
+
+// Camera checkpoint score -- the losses of cam_est/model_cam.py:125-239 that eval_one_epoch (cam_est/
+// train_sdf_cam.py:459-565) fetches, per image.  Per point p, with h = [p, 1] and every matrix product summed in k order:
+//   sub = h.pred_RT - h.RT                                     -> sums[0] += |sub|^2 (element by element), sums[2] += sqrt(|sub|^2)
+//   xy = (h.tm)[:2] / (h.tm)[2] for tm and pred_tm (get_img_points) -> sums[1] += |xy_pr - xy_gt|^2 (element by element),
+//        sums[3] += sqrt(|clamp(xy_gt) - clamp(xy_pr)|^2) with the reference's hard-coded [0, 136] clamp
+// and sums[4] = sum over the 12 entries of (pred_tm - tm)^2.  The terms are float32, one rounding per op (this file is
+// built with --fmad=false); the sums are float64 in a fixed order (thread-strided loop, then a fixed tree), so repeated
+// calls are bitwise equal.
+constexpr int CAM_ACC_THREADS = 256;
+
+__device__ __forceinline__ void homo_mul(const float* p, const float* M, float* out) {   // [p, 1] . M[4,3]
+  for (int j = 0; j < 3; ++j) out[j] = ((p[0] * M[j] + p[1] * M[3 + j]) + p[2] * M[6 + j]) + M[9 + j];
+}
+
+__device__ __forceinline__ float clamp136(float x) { return fminf(136.f, fmaxf(0.f, x)); }
+
+__global__ void __launch_bounds__(CAM_ACC_THREADS) cam_acc_kernel(const float* __restrict__ pts, int64_t N,
+                                                                  const float* __restrict__ tm, const float* __restrict__ rt,
+                                                                  const float* __restrict__ pred_tm,
+                                                                  const float* __restrict__ pred_rt,
+                                                                  double* __restrict__ sums) {
+  __shared__ float m[4][12];      // tm, RT, pred_tm, pred_RT of this image
+  __shared__ double s[4][CAM_ACC_THREADS];
+  const int b = blockIdx.x, t = threadIdx.x;
+  if (t < 48) {
+    const float* src = t < 12 ? tm : t < 24 ? rt : t < 36 ? pred_tm : pred_rt;
+    m[t / 12][t % 12] = src[(size_t)b * 12 + t % 12];
+  }
+  __syncthreads();
+  const float* P = pts + (size_t)b * N * 3;
+  double rotpc = 0.0, rot2d = 0.0, rot3d = 0.0, dist2d = 0.0;
+  for (int64_t n = t; n < N; n += CAM_ACC_THREADS) {
+    const float p[3] = {P[3 * n], P[3 * n + 1], P[3 * n + 2]};
+    float a[3], g[3], u[3], v[3];
+    homo_mul(p, m[3], a);
+    homo_mul(p, m[1], g);
+    const float s0 = a[0] - g[0], s1 = a[1] - g[1], s2 = a[2] - g[2];
+    const float q0 = s0 * s0, q1 = s1 * s1, q2 = s2 * s2;
+    rotpc = ((rotpc + (double)q0) + (double)q1) + (double)q2;
+    rot3d += (double)sqrtf((q0 + q1) + q2);
+    homo_mul(p, m[0], u);
+    homo_mul(p, m[2], v);
+    const float xg = u[0] / u[2], yg = u[1] / u[2], xp = v[0] / v[2], yp = v[1] / v[2];
+    const float dx = xp - xg, dy = yp - yg;
+    rot2d = (rot2d + (double)(dx * dx)) + (double)(dy * dy);
+    const float cx = clamp136(xg) - clamp136(xp), cy = clamp136(yg) - clamp136(yp);
+    dist2d += (double)sqrtf(cx * cx + cy * cy);
+  }
+  s[0][t] = rotpc; s[1][t] = rot2d; s[2][t] = rot3d; s[3][t] = dist2d;
+  __syncthreads();
+  for (int h = CAM_ACC_THREADS / 2; h > 0; h >>= 1) {
+    if (t < h)
+      for (int k = 0; k < 4; ++k) s[k][t] += s[k][t + h];
+    __syncthreads();
+  }
+  if (t == 0) {
+    double mat = 0.0;
+    for (int i = 0; i < 12; ++i) {
+      const float d = m[2][i] - m[0][i];
+      mat += (double)(d * d);
+    }
+    for (int k = 0; k < 4; ++k) sums[(size_t)b * 5 + k] = s[k][0];
+    sums[(size_t)b * 5 + 4] = mat;
+  }
+}
+
+}  // namespace
 }  // namespace disn
+
+using namespace disn;
+
+extern "C" int disn_cam_metrics(disn_ctx* c, const float* imgs, int32_t B, int32_t H, int32_t W, int32_t C, const float* K,
+                                const float* pts, int64_t N, const float* trans_mat, const float* RT, float* out_rt,
+                                float* out_trans_mat, double* sums) {
+  DISN_REQUIRE(c && imgs && pts && trans_mat && RT && sums, "null argument");
+  DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
+  DISN_REQUIRE(B >= 1 && B <= c->cfg.max_batch, "cam_metrics: batch outside [1, max_batch of the context]");
+  DISN_REQUIRE(N >= 1, "cam_metrics: N >= 1 points per image");
+  float *dK, *dRT, *dTM, *dPts, *dGtTM, *dGtRT;
+  double* dSums;
+  auto carve = [&](char* base) {
+    Arena a{base};
+    dK = a.take<float>(9);
+    dRT = a.take<float>((size_t)B * 12);
+    dTM = a.take<float>((size_t)B * 12);
+    dGtRT = a.take<float>((size_t)B * 12);
+    dGtTM = a.take<float>((size_t)B * 12);
+    dSums = a.take<double>((size_t)B * 5);
+    dPts = a.take<float>((size_t)B * N * 3);
+    return a.off;
+  };
+  if (c->nn_scratch.ensure(carve(nullptr))) return -1;
+  carve(c->nn_scratch.as<char>());
+  if (cam_predict(c, imgs, B, H, W, C, K, dK, dRT, dTM)) return -1;
+  DISN_CUDA_OK(cudaMemcpyAsync(dPts, pts, (size_t)B * N * 3 * 4, cudaMemcpyHostToDevice, c->stream));
+  DISN_CUDA_OK(cudaMemcpyAsync(dGtTM, trans_mat, (size_t)B * 12 * 4, cudaMemcpyHostToDevice, c->stream));
+  DISN_CUDA_OK(cudaMemcpyAsync(dGtRT, RT, (size_t)B * 12 * 4, cudaMemcpyHostToDevice, c->stream));
+  cam_acc_kernel<<<B, CAM_ACC_THREADS, 0, c->stream>>>(dPts, N, dGtTM, dGtRT, dTM, dRT, dSums);
+  c->launches++;
+  DISN_CUDA_OK(cudaGetLastError());
+  if (out_rt) DISN_CUDA_OK(cudaMemcpyAsync(out_rt, dRT, (size_t)B * 12 * 4, cudaMemcpyDeviceToHost, c->stream));
+  if (out_trans_mat) DISN_CUDA_OK(cudaMemcpyAsync(out_trans_mat, dTM, (size_t)B * 12 * 4, cudaMemcpyDeviceToHost, c->stream));
+  DISN_CUDA_OK(cudaMemcpyAsync(sums, dSums, (size_t)B * 5 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
+  return 0;
+}

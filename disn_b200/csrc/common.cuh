@@ -407,6 +407,10 @@ int launch_conv_tc(disn_ctx* c, const float* A, const uint8_t* wpk, const float*
 // cam.cu
 // the pose heads on the embeddings d_emb [B, num_classes] (device) -> pred_RT and pred_trans_mat [B,4,3] (device)
 int launch_cam_heads(disn_ctx* c, int B, const float* d_emb, const float* d_K, float* d_rt, float* d_tm);
+// the embedding-only encode of host imgs [B,H,W,C], then the heads with intrinsics K (host float[9], NULL = the reference's
+// constant) staged in d_K: pred_RT and pred_trans_mat [B,4,3] in the caller's device buffers (disn_cam_estimate/_metrics)
+int cam_predict(disn_ctx* c, const float* imgs, int B, int H, int W, int C, const float* K, float* d_K, float* d_rt,
+                float* d_tm);
 // chamfer.cu
 int nn_distance(disn_ctx* c, const float* d_xyz1, int n, const float* d_xyz2, int m, int B, float* d_dist1,
                 int* d_idx1, float* d_dist2, int* d_idx2);

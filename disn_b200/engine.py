@@ -241,6 +241,24 @@ class Engine:
                                          tm.ctypes.data_as(C.c_void_p)))
         return (tm, rt) if want_rt else tm
 
+    def cam_metrics(self, imgs, pts, trans_mat, RT, K=None):
+        """The camera checkpoint score of cam_est/train_sdf_cam.py --test (disn_cam_metrics): imgs [B,H,W,3], pts
+        [B,N,3], ground-truth trans_mat and RT (the view file's regress_mat) [B,4,3] -> (pred_trans_mat [B,4,3], pred_RT
+        [B,4,3], sums float64 [B,5]).  The predictions are cam_estimate's bits; cam_losses turns the sums into the batch
+        values."""
+        a, p, t, r = _f32(imgs), _f32(pts), _f32(trans_mat), _f32(RT)
+        if a.ndim != 4 or p.ndim != 3 or p.shape[2] != 3:
+            raise ValueError("imgs must be [B,H,W,C] and pts [B,N,3]")
+        B, H, W, Cc = a.shape
+        if p.shape[0] != B or t.size != B * 12 or r.size != B * 12:
+            raise ValueError("pts, trans_mat and RT must hold one entry per image")
+        tm, rt, sums = np.empty((B, 4, 3), np.float32), np.empty((B, 4, 3), np.float32), np.empty((B, 5), np.float64)
+        kk = None if K is None else _f32(K).reshape(9)
+        ptr = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)
+        check(self.lib.disn_cam_metrics(self._h, ptr(a), B, H, W, Cc, ptr(kk), ptr(p), p.shape[1], ptr(t), ptr(r), ptr(rt),
+                                        ptr(tm), ptr(sums)))
+        return tm, rt, sums
+
     def load_weights_raw(self, weights: dict):
         """Upload variables without finalising the SDF heads (camera-net contexts have no sdfprediction/*)."""
         for name, arr in weights.items():
@@ -693,6 +711,38 @@ def batch_losses(count, wsum, rsum, n_values: int):
     real = np.float32(float(np.sum(rsum)) / n_values)
     loss = np.float32(float(np.sum(wsum)) / n_values) * np.float32(1000)
     return acc, real, loss
+
+
+CAM_LOSS_KEYS = ("rotpc_loss", "rot2d_loss", "rot3d_dist", "rot2d_dist", "rotmatrix_loss", "regularization",
+                 "overall_loss")
+
+
+def cam_losses(sums, n_points: int, regularization, loss_mode: str = "3D"):
+    """The losses of cam_est/model_cam.py get_loss (:153-237) from per-image cam_metrics sums [B,5] over n_points points
+    per image: (dict of float32 in CAM_LOSS_KEYS order, rot3d_dist_all [B], rot2d_dist_all [B]).  overall_loss follows
+    --loss_mode: 3D rotpc, 2D rot2d, 3DM rotpc + 0.3 rotmatrix, anything else rot2d + rotpc + rotmatrix; plus the
+    regularization constant of the checkpoint."""
+    s = np.asarray(sums, np.float64).reshape(-1, 5)
+    B = len(s)
+    f32 = np.float32
+    rotpc = f32(float(np.sum(s[:, 0])) / 2)                                   # l2_loss = sum / 2
+    rot2d = f32(float(np.sum(s[:, 1])) / 2) / f32(10000.)
+    rot3d_all = (s[:, 2] / n_points).astype(np.float32)                       # reduce_mean over the points
+    rot2d_all = (s[:, 3] / n_points).astype(np.float32)
+    rot3d = f32(np.mean(rot3d_all, dtype=np.float64))
+    rot2d_dist = f32(np.mean(rot2d_all, dtype=np.float64))
+    rotmatrix = f32(float(np.sum(s[:, 4])) / (12 * B))
+    if loss_mode == "3D":
+        loss = rotpc
+    elif loss_mode == "2D":
+        loss = rot2d
+    elif loss_mode == "3DM":
+        loss = rotpc + rotmatrix * f32(0.3)
+    else:
+        loss = rot2d + rotpc + rotmatrix
+    reg = f32(regularization)
+    vals = (rotpc, rot2d, rot3d, rot2d_dist, rotmatrix, reg, f32(loss + reg))
+    return dict(zip(CAM_LOSS_KEYS, vals)), rot3d_all, rot2d_all
 
 
 def write_dist(path: str, res: int, bbox, values):

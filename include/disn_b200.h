@@ -287,6 +287,20 @@ int disn_sdf_strided(disn_ctx* ctx, const float* sdf, int32_t R, int32_t reduce,
 int disn_cam_estimate(disn_ctx* ctx, const float* imgs, int32_t B, int32_t H, int32_t W, int32_t C, const float* K,
                       float* out_rt, float* out_trans_mat);
 
+/* Camera checkpoint score (cam_est/train_sdf_cam.py:459-565 eval_one_epoch, cam_est/model_cam.py:111-239): the
+ * prediction of disn_cam_estimate on imgs, then per image b over the N points pts [B,N,3] (host float32) with the ground
+ * truth trans_mat and RT (the view file's regress_mat) [B,4,3], h = [p, 1]:
+ *   sums[b][0] = sum |h.pred_RT - h.RT|^2                          (rotpc_loss = total / 2)
+ *   sums[b][1] = sum |xy_pred - xy_gt|^2, xy = (h.M)[:2] / (h.M)[2] (rot2d_loss = total / 2 / 10000)
+ *   sums[b][2] = sum sqrt(|h.pred_RT - h.RT|^2)                    (rot3d_dist_all = sums[b][2] / N)
+ *   sums[b][3] = sum sqrt(|clamp(xy_gt) - clamp(xy_pred)|^2), clamp to [0, 136]  (rot2d_dist_all = sums[b][3] / N)
+ *   sums[b][4] = sum over the 12 entries of (pred_trans_mat - trans_mat)^2     (rotmatrix_loss = total / (12 B))
+ * Float32 terms, one rounding per op; float64 sums in a fixed order (repeated calls are bitwise equal).  out_rt and
+ * out_trans_mat (either may be NULL) receive disn_cam_estimate's bits.  B in [1, max_batch], N >= 1. */
+int disn_cam_metrics(disn_ctx* ctx, const float* imgs, int32_t B, int32_t H, int32_t W, int32_t C, const float* K,
+                     const float* pts, int64_t N, const float* trans_mat, const float* RT, float* out_rt,
+                     float* out_trans_mat, double* sums);
+
 /* Chamfer nearest-neighbour distances, the reference's NnDistance op (models/tf_ops/nn_distance/tf_nndistance.cpp:
  * 21-43; called at test/test_cd_emd.py:300, test/test_f_score.py:253): xyz1 [B,N,3], xyz2 [B,M,3] host float32 ->
  * dist1 [B,N] (squared L2 to the nearest point of xyz2), idx1 [B,N] int32, dist2 [B,M], idx2 [B,M].
