@@ -112,10 +112,11 @@ static_assert(ptc::store_offset_mismatches() == 0, "epilogue / prologue store of
 // of kMode: the 2-byte pair at byte offset o16 (ptc::epi_off16 / pro_off16), MODE_F16F8's e5m2 pairs at o8
 // (ptc::epi_off8 / pro_off8).  MODE_F16F8 also folds the fp16 values into `amax` (all values are post-ReLU, i.e. >= 0):
 // an activation above fp16's 65504 becomes +inf there, which the kernel reports through PointJob::status instead of
-// producing a silent inf.
+// producing a silent inf.  `copy`: MODE_F16F8 also stores the e5m2 copy, which only the consuming layer's second
+// correction product reads (a compile-time constant after inlining).
 template <int kMode>
 __device__ __forceinline__ void store_pair(uint8_t* x, uint32_t o16, uint32_t o8, float a, float b, float sc_lo,
-                                           float sc_hi, __half2& amax) {
+                                           float sc_hi, __half2& amax, bool copy) {
   if constexpr (kMode == MODE_BF16X3) {
     uint32_t hi, lo;
     tc::split_bf16x2(a, b, hi, lo);
@@ -127,10 +128,13 @@ __device__ __forceinline__ void store_pair(uint8_t* x, uint32_t o16, uint32_t o8
     *reinterpret_cast<__half2*>(x + o16) = hh;
     const float ra = a - __low2float(hh), rb = b - __high2float(hh);      // fp16 rounding residual (first correction)
     const __nv_fp8x2_storage_t l = __nv_cvt_float2_to_fp8x2(make_float2(ra * sc_lo, rb * sc_lo), __NV_SATFINITE, __NV_E5M2);
-    const __half2 hs = __hmul2(hh, __float2half2_rn(sc_hi));   // power-of-two scale: exact up to fp16 underflow
-    const __nv_fp8x2_storage_t g = __nv_cvt_halfraw2_to_fp8x2(*reinterpret_cast<const __half2_raw*>(&hs), __NV_SATFINITE, __NV_E5M2);
     *reinterpret_cast<__nv_fp8x2_storage_t*>(x + o8) = l;
-    *reinterpret_cast<__nv_fp8x2_storage_t*>(x + o8 + X8_TILE) = g;
+    if (copy) {
+      const __half2 hs = __hmul2(hh, __float2half2_rn(sc_hi));   // power-of-two scale: exact up to fp16 underflow
+      const __nv_fp8x2_storage_t g =
+          __nv_cvt_halfraw2_to_fp8x2(*reinterpret_cast<const __half2_raw*>(&hs), __NV_SATFINITE, __NV_E5M2);
+      *reinterpret_cast<__nv_fp8x2_storage_t*>(x + o8 + X8_TILE) = g;
+    }
   }
 }
 
@@ -222,7 +226,7 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
             v2[e] = fmaxf(a, 0.f);
           }
           store_pair<kMode>(s.x[0], ptc::pro_off16(o16, j), ptc::pro_off8(o8, j), v2[0], v2[1], job.act_scale[sx][0][0],
-                            job.act_scale[sx][0][1], amax);
+                            job.act_scale[sx][0][1], amax, ((kC >> 1) & 1) != 0);
         }
       }
       tc::fence_proxy_async_smem();
@@ -240,37 +244,39 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
             const uint32_t slot = g % NSLOT, par = (ph >> slot) & 1u;
             tc::mbar_wait(&full[slot][h], par);
             ph ^= 1u << slot;
-            const uint32_t xa = x_base + (uint32_t)t * X_SLICE, wb = w_base + slot * HS_BYTES;
+            // descriptor low words of the slice's A tile and the slot's B tile; every other operand of the half-stage is
+            // a constant number of 16-byte units (>> 4) further (tc::desc_lo)
+            const uint32_t xa = tc::desc_lo(x_base + (uint32_t)t * X_SLICE), wb = tc::desc_lo(w_base + slot * HS_BYTES);
             tc::acc_fence(acc[nb]);
             if constexpr (kMode == MODE_F16F8) tc::acc_fence(tmp);
             tc::wgmma_fence();
             if constexpr (kMode == MODE_BF16X3) {
 #pragma unroll
               for (int k = 0; k < 4; ++k)
-                tc::wgmma_m64n128<tc::KIND_BF16>(acc[nb], tc::desc_sw128(xa + 32u * k), tc::desc_sw128(wb + 32u * k), (t | k) ? 1u : 0u);
+                tc::wgmma_m64n128_lo<tc::KIND_BF16>(acc[nb], xa + 2u * k, wb + 2u * k, (t | k) ? 1u : 0u);
 #pragma unroll
               for (int k = 0; k < 4; ++k)
-                tc::wgmma_m64n128<tc::KIND_BF16>(acc[nb], tc::desc_sw128(xa + X_TILE + 32u * k), tc::desc_sw128(wb + 32u * k), 1u);
+                tc::wgmma_m64n128_lo<tc::KIND_BF16>(acc[nb], xa + (X_TILE >> 4) + 2u * k, wb + 2u * k, 1u);
 #pragma unroll
               for (int k = 0; k < 4; ++k)
-                tc::wgmma_m64n128<tc::KIND_BF16>(acc[nb], tc::desc_sw128(xa + 32u * k), tc::desc_sw128(wb + W_TILE + 32u * k), 1u);
+                tc::wgmma_m64n128_lo<tc::KIND_BF16>(acc[nb], xa + 2u * k, wb + (W_TILE >> 4) + 2u * k, 1u);
             } else {
 #pragma unroll
               for (int k = 0; k < 4; ++k)
-                tc::wgmma_m64n128<tc::KIND_F16>(acc[nb], tc::desc_sw128(xa + 32u * k), tc::desc_sw128(wb + 32u * k), (t | k) ? 1u : 0u);
+                tc::wgmma_m64n128_lo<tc::KIND_F16>(acc[nb], xa + 2u * k, wb + 2u * k, (t | k) ? 1u : 0u);
               // corrections into the zero-initialised side accumulator, in the same commit group; they are added after
               // the wait, so each element still gets main(t), then + corr(t), then main(t + 1)
               if (k1) {
 #pragma unroll
                 for (int k = 0; k < 2; ++k)
-                  tc::wgmma_m64n128<tc::KIND_E5M2>(tmp, tc::desc_sw64(xa + X_TILE + 32u * k), tc::desc_sw64(wb + W_TILE + 32u * k),
-                                                   k ? 1u : 0u);
+                  tc::wgmma_m64n128_lo<tc::KIND_E5M2>(tmp, xa + (X_TILE >> 4) + 2u * k, wb + (W_TILE >> 4) + 2u * k,
+                                                      k ? 1u : 0u);
               }
               if (k2) {
 #pragma unroll
                 for (int k = 0; k < 2; ++k)
-                  tc::wgmma_m64n128<tc::KIND_E5M2>(tmp, tc::desc_sw64(xa + X_TILE + X8_TILE + 32u * k),
-                                                   tc::desc_sw64(wb + W_TILE + W8_TILE + 32u * k), (k1 || k) ? 1u : 0u);
+                  tc::wgmma_m64n128_lo<tc::KIND_E5M2>(tmp, xa + ((X_TILE + X8_TILE) >> 4) + 2u * k,
+                                                      wb + ((W_TILE + W8_TILE) >> 4) + 2u * k, (k1 || k) ? 1u : 0u);
               }
             }
             tc::wgmma_commit();
@@ -298,6 +304,8 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
         if (layer < 3) {
           // ---- epilogue: bias (+ folded image features), ReLU, operand split -> next layer's input, in place
           const bool gather = (sx == 1 && layer == 2);
+          // the next layer reads the e5m2 copy only if it keeps the second correction (not fold2/conv1 by default)
+          const bool copy = ((kC >> (2 * layer + 3)) & 1) != 0;
           int off[2][4];
           float wg[2][4];
           if (gather) {
@@ -357,7 +365,7 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
                 const float va = fmaxf(acc[nb][4 * j + 2 * e2] + v2[0], 0.f);
                 const float vb = fmaxf(acc[nb][4 * j + 2 * e2 + 1] + v2[1], 0.f);
                 store_pair<kMode>(s.x[0], ptc::epi_off16(base16, nb, j, e2), ptc::epi_off8(base8, nb, j, e2), va, vb,
-                                  sc_lo, sc_hi, amax);
+                                  sc_lo, sc_hi, amax, copy);
               }
             }
           }

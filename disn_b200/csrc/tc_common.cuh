@@ -179,6 +179,39 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t da, uint6
   }
 }
 
+// Low word of a descriptor (start address >> 4 and the leading byte offset); the high word is a constant per swizzle
+// mode.  Moving the start address by `off` bytes (a multiple of 16, staying inside shared memory, whose addresses
+// fit the 14-bit field) adds off >> 4 to it, so the descriptors of one operand tile are one add apart.
+__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr) { return ((smem_addr >> 4) & 0x3FFFu) | (1u << 16); }
+
+// wgmma_m64n128 with both operands given by descriptor low words: SW128 (KIND_BF16, KIND_F16) or SW64 (KIND_E5M2)
+// tiles.  The 64-bit descriptors are formed inside the asm from the constant high word, so the compiler does no
+// 64-bit descriptor arithmetic per instruction.
+template <int kKind>
+__device__ __forceinline__ void wgmma_m64n128_lo(float (&d)[64], uint32_t da, uint32_t db, uint32_t accumulate) {
+  constexpr uint32_t hi = kKind == KIND_E5M2 ? kDescHiSw64 : kDescHiSw128;
+#define DISN_WGMMA_LO_PRE                                                                                        \
+  "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                         \
+  "mov.b64 da, {%64, %67};\n\tmov.b64 db, {%65, %67};\n\t"
+  if constexpr (kKind == KIND_BF16) {
+    asm volatile(DISN_WGMMA_LO_PRE
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " DISN_WGMMA_D64 ", da, db, p, 1, 1, 0, 0;\n\t}"
+                 : DISN_WGMMA_OPS64
+                 : "r"(da), "r"(db), "r"(accumulate), "r"(hi));
+  } else if constexpr (kKind == KIND_F16) {
+    asm volatile(DISN_WGMMA_LO_PRE
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " DISN_WGMMA_D64 ", da, db, p, 1, 1, 0, 0;\n\t}"
+                 : DISN_WGMMA_OPS64
+                 : "r"(da), "r"(db), "r"(accumulate), "r"(hi));
+  } else {
+    asm volatile(DISN_WGMMA_LO_PRE
+                 "wgmma.mma_async.sync.aligned.m64n128k32.f32.e5m2.e5m2 " DISN_WGMMA_D64 ", da, db, p, 1, 1;\n\t}"
+                 : DISN_WGMMA_OPS64
+                 : "r"(da), "r"(db), "r"(accumulate), "r"(hi));
+  }
+#undef DISN_WGMMA_LO_PRE
+}
+
 #undef DISN_WGMMA_D64
 #undef DISN_WGMMA_OPS64
 
