@@ -25,6 +25,11 @@ class DisnConfig(C.Structure):
                 ("tanh_out", C.c_int32), ("precision", C.c_int32), ("max_batch", C.c_int32)]
 
 
+class DisnTrainConfig(C.Structure):
+    _fields_ = [("beta1", C.c_float), ("beta2", C.c_float), ("epsilon", C.c_float), ("wd", C.c_float),
+                ("mask_weight", C.c_float), ("sdf_weight", C.c_float)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "disn_default_config": (None, [C.POINTER(DisnConfig)]),
@@ -102,6 +107,14 @@ EXPORTS = {
     "disn_obj_read_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "disn_sdf_metrics": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_float,
                                    C.c_float, C.c_float, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "disn_default_train_config": (None, [C.POINTER(DisnTrainConfig)]),
+    "disn_train_begin": (C.c_int, [C.c_void_p, C.POINTER(DisnTrainConfig)]),
+    "disn_train_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_void_p]),
+    "disn_train_get": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
+    "disn_train_set": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
+    "disn_train_var_name": (C.c_int, [C.c_int32, C.c_char_p, C.c_int64]),
+    "disn_train_phase_ms": (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
 }
 
 # diagnostics (include/disn_b200_test.h), exported by libdisn_b200_test.so only
@@ -126,6 +139,9 @@ TEST_EXPORTS = {
     "disn_mesh_adaptive_edges": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
     "disn_debug_obj_tokens": (C.c_int, [C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "disn_debug_cam_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "disn_debug_train_grads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]),
 }
 
 _lib = None

@@ -11,8 +11,9 @@ LIB = os.path.join(HERE, "libdisn_b200.so")
 TEST_LIB = os.path.join(HERE, "libdisn_b200_test.so")
 SOURCES = ["api.cu", "encoder.cu", "point_fp32.cu", "point_tc.cu", "mc.cu", "chamfer.cu", "conv_tc.cu", "cam.cu", "iou.cu",
            "decoder.cu", "emd.cu", "mesh_clean.cu", "mesh_sdf.cu", "mesh_normalize.cu", "sdf_sample.cu", "adaptive.cu",
-           "adaptive_mesh.cu", "obj_read.cu", "sdf_acc.cu"]
-# diagnostics: selftests / probes, plus encoder.cu rebuilt with its debug GEMM harness -> libdisn_b200_test.so
+           "adaptive_mesh.cu", "obj_read.cu", "sdf_acc.cu", "decoder_train.cu"]
+# diagnostics: selftests / probes, plus encoder.cu and decoder_train.cu rebuilt with their debug harnesses
+# -> libdisn_b200_test.so
 DIAG_SOURCES = ["tc_selftest.cu", "tc_probe.cu", "adaptive_diag.cu", "tc_diag.cu", "obj_diag.cu", "cam_diag.cu"]
 # voxel classification (iou.cu), the small-part keep rule (mesh_clean.cu) and the distances and edge crossings of the
 # signed distance field (mesh_sdf.cu) and the face areas, surface samples and normalised vertices (mesh_normalize.cu) must
@@ -50,10 +51,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
     from concurrent.futures import ThreadPoolExecutor
     jobs = [(src, os.path.join(CSRC, src.replace(".cu", ".o")), EXTRA_FLAGS.get(src, [])) for src in SOURCES + DIAG_SOURCES]
     jobs.append(("encoder.cu", os.path.join(CSRC, "encoder_diag.o"), ["-DDISN_DIAGNOSTICS"]))
+    jobs.append(("decoder_train.cu", os.path.join(CSRC, "decoder_train_diag.o"), ["-DDISN_DIAGNOSTICS"]))
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(lambda j: _compile(j[0], j[1], j[2], verbose), jobs))
     prod = objs[:len(SOURCES)]
-    diag = [o for o in prod if not o.endswith("encoder.o")] + objs[len(SOURCES):]
+    diag = [o for o in prod if not o.endswith(("encoder.o", "decoder_train.o"))] + objs[len(SOURCES):]
     for out, oo in ((LIB, prod), (TEST_LIB, diag)):
         r = subprocess.run([NVCC, "-shared", "-o", out] + oo + ["-lcudart"], capture_output=True, text=True)
         if r.returncode != 0:

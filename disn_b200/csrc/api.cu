@@ -212,13 +212,14 @@ int disn_encode(disn_ctx* c, const float* imgs, int32_t B, int32_t H, int32_t W,
   DISN_REQUIRE(B <= c->cfg.max_batch, "batch exceeds max_batch of the context");
   if (c->weights_dirty && disn_finalize_weights(c)) return -1;
   if (encoder_run(c, imgs, B, H, W, C, (flags & DISN_DEVICE_PTR) != 0)) return -1;
+  c->enc_stale = false;
   if (!(flags & DISN_DEVICE_PTR)) DISN_CUDA_OK(cudaStreamSynchronize(c->stream));   // caller-owned host buffer
   return 0;
 }
 
 int disn_get_encoded(disn_ctx* c, int32_t what, float* out, int64_t out_elems) {
   DISN_REQUIRE(c && out, "null ctx/out");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
   static const int tapHW[5] = {224, 112, 56, 28, 14};
   const float* src = nullptr;
@@ -285,7 +286,7 @@ extern "C" {
 int disn_eval_points(disn_ctx* c, const float* pts, const float* pts_rot, const float* trans_mat, int32_t B,
                      int64_t N, float* out_pred, float* out_uv, uint32_t flags) {
   DISN_REQUIRE(c && pts && trans_mat && out_pred, "null argument");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_REQUIRE(B == c->enc_B, "batch differs from the encoded batch");
   DISN_REQUIRE(N >= 0, "negative N");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
@@ -340,7 +341,7 @@ static void linspace_f32(double start, double stop, int num, float* out) {
 int disn_eval_grid(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t B, int32_t sdf_res,
                    int32_t z0, int32_t z1, float* out_sdf, uint32_t flags) {
   DISN_REQUIRE(c && sdf_params && trans_mat && out_sdf, "null argument");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_REQUIRE(B == c->enc_B, "batch differs from the encoded batch");
   DISN_REQUIRE(sdf_res >= 1, "sdf_res >= 1");
   const int R = sdf_res + 1;
@@ -631,7 +632,7 @@ int disn_eval_grid_resident(disn_ctx* c, const double* sdf_params, const float* 
 int disn_eval_grid_indexed(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t image, int32_t sdf_res,
                            const int32_t* idx, int64_t n, float* out, uint32_t flags) {
   DISN_REQUIRE(c && sdf_params && trans_mat && ((idx && out) || n == 0), "null argument");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_REQUIRE(image >= 0 && image < c->enc_B, "image outside the encoded batch");
   DISN_REQUIRE(sdf_res >= 1 && (int64_t)(sdf_res + 1) * (sdf_res + 1) * (sdf_res + 1) <= INT32_MAX,
                "eval_grid_indexed: 1 <= sdf_res and (sdf_res+1)^3 < 2^31");
@@ -657,7 +658,7 @@ int disn_eval_grid_indexed(disn_ctx* c, const double* sdf_params, const float* t
 int disn_eval_grid_adaptive(disn_ctx* c, const double* sdf_params, const float* trans_mat, int32_t image, int32_t sdf_res,
                             float iso, double band, float** grid_dev, int64_t* level_counts, int32_t* n_levels) {
   DISN_REQUIRE(c && sdf_params && trans_mat && grid_dev && level_counts && n_levels, "null argument");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_REQUIRE(image >= 0 && image < c->enc_B, "image outside the encoded batch");
   DISN_REQUIRE(sdf_res >= 1 && (int64_t)(sdf_res + 1) * (sdf_res + 1) * (sdf_res + 1) <= INT32_MAX,
                "eval_grid_adaptive: 1 <= sdf_res and (sdf_res+1)^3 < 2^31");
@@ -695,7 +696,7 @@ int disn_mesh_grid_adaptive(disn_ctx* c, const double* sdf_params, const float* 
                             float iso, double band, int64_t* level_counts, int32_t* n_levels, int64_t* n_verts,
                             int64_t* n_faces) {
   DISN_REQUIRE(c && sdf_params && trans_mat && level_counts && n_levels, "null argument");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_REQUIRE(image >= 0 && image < c->enc_B, "image outside the encoded batch");
   DISN_REQUIRE(sdf_res >= 1 && sdf_res <= 2048, "mesh_grid_adaptive: 1 <= sdf_res <= 2048");
   DISN_REQUIRE(std::isfinite(iso), "mesh_grid_adaptive: iso must be finite");

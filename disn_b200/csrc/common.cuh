@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include <map>
+#include <memory>
 #include <set>
 #include <string>
 #include <utility>
@@ -266,6 +267,10 @@ class ResidentMesh {
   int64_t nv_ = 0, nf_ = 0;
 };
 
+struct TrainState;    // decoder training (decoder_train.cu)
+void train_state_free(TrainState* t);
+struct TrainStateDeleter { void operator()(TrainState* t) const { train_state_free(t); } };
+
 }  // namespace disn
 
 // Every allocation of the context is a buffer member: deleting the context frees them all.
@@ -379,9 +384,19 @@ struct disn_ctx {
   disn::DevBuffer nn_scratch;
   disn::DevBuffer dec_scratch;  // explicit-feature decoder staging (decoder.cu)
   disn::DevBuffer d_gt, d_acc;  // disn_sdf_metrics: host-call staging of the samples' values and the per-image sums
+  // decoder training (decoder_train.cu): Adam slots, gradients and step scratch; null until disn_train_begin.  enc_stale:
+  // a training step changed the decoder since the last disn_encode, so the encoded state was dropped
+  std::unique_ptr<disn::TrainState, disn::TrainStateDeleter> train;
+  bool enc_stale = false;
 };
 
 namespace disn {
+// the error of a call that needs the encoded state when there is none
+inline std::string not_encoded(const disn_ctx* c) {
+  return c->enc_stale ? "the encoded state is stale: a training step changed the decoder weights since the last "
+                        "disn_encode; call disn_encode again"
+                      : "disn_encode has not been called";
+}
 // encoder.cu
 int encoder_alloc(disn_ctx* c, int B);
 int encoder_run(disn_ctx* c, const float* imgs, int B, int H, int W, int C, bool device_ptr,
@@ -395,6 +410,10 @@ int check_status(disn_ctx* c);    // after a synchronisation: the kernels' statu
 int encoder_gemv(disn_ctx* c, const float* x, const float* W, const float* bias, float* out, int B, int K, int N, int relu);
 int encoder_gemm_plain(disn_ctx* c, const std::string& wname, const float* A, const float* Bm, const float* bias, float* C,
                        int M, int N, int K, int relu);
+// decoder.cu: the 1472 point features of the encoded batch at d_pts [B,N,3] through d_tm [B,4,3] (device) -> d_uv [B,N,2]
+// and rows of `out` ld floats apart
+int gather_point_feat(disn_ctx* c, const float* d_pts, const float* d_tm, int B, int64_t N, float* d_uv, float* out,
+                      int64_t ld);
 // point_fp32.cu
 int launch_point_fp32(disn_ctx* c, const PointJob& job);
 // point_tc.cu
@@ -402,6 +421,10 @@ int tc_pack_weights(disn_ctx* c);
 int launch_point_tc(disn_ctx* c, const PointJob& job);
 // conv_tc.cu
 int conv_tc_pack(disn_ctx* c, const float* d_w, int K, int N, DevBuffer& out);
+// the same stage images packed on the device, on c->stream: element (k, n) of the [K, N] operand is src[k * ld + n], or
+// src[n * ld + k] with trans; out must hold conv_tc_packed_bytes(K, N)
+size_t conv_tc_packed_bytes(int K, int N);
+int conv_tc_pack_device(disn_ctx* c, const float* src, int K, int N, int64_t ld, bool trans, uint8_t* out);
 int launch_conv_tc(disn_ctx* c, const float* A, const uint8_t* wpk, const float* bias, float* C, float* ws,
                    int64_t ws_elems, int M, int N, int K, int H, int W, int Cin, int relu, int* splits_out);
 // cam.cu

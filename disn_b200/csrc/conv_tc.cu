@@ -17,6 +17,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
 #include <cstring>
 #include <vector>
 
@@ -205,6 +206,45 @@ int conv_tc_pack(disn_ctx* c, const float* d_w, int K, int N, DevBuffer& out) {
   if (out.ensure(img.size())) return -1;
   DISN_CUDA_OK(cudaMemcpyAsync(out.as<uint8_t>(), img.data(), img.size(), cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+size_t conv_tc_packed_bytes(int K, int N) { return (size_t)((N + 127) / 128) * (K / 64) * CT_B_STAGE; }
+
+namespace {
+// one thread per (n-block, k-slice, hi|lo, row, 8-k group): 16 bytes of one stage image, conv_tc_pack's bytes
+__global__ void conv_tc_pack_kernel(const float* __restrict__ src, int K, int N, int64_t ld, int trans,
+                                    uint8_t* __restrict__ out) {
+  const int ns = K / 64;
+  const int64_t total = (int64_t)((N + 127) / 128) * ns * 2 * 128 * 8;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i & 7), nl = (int)((i >> 3) & 127), part = (int)((i >> 10) & 1);
+    const int64_t st = i >> 11;                 // nb * ns + t
+    const int nb = (int)(st / ns), t = (int)(st % ns);
+    const int n = nb * 128 + nl;
+    uint16_t h[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = t * 64 + g * 8 + j;
+      const float v = n < N ? (trans ? src[(int64_t)n * ld + k] : src[(int64_t)k * ld + n]) : 0.f;
+      const __nv_bfloat16 hi = __float2bfloat16(v);
+      const __nv_bfloat16 o = part == 0 ? hi : __float2bfloat16(v - __bfloat162float(hi));
+      h[j] = __bfloat16_as_ushort(o);
+    }
+    uint8_t* dst = out + st * CT_B_STAGE + (size_t)part * CT_B_TILE + tc::sw128_offset(nl, g);
+    *reinterpret_cast<uint4*>(dst) = make_uint4(h[0] | (uint32_t)h[1] << 16, h[2] | (uint32_t)h[3] << 16,
+                                                h[4] | (uint32_t)h[5] << 16, h[6] | (uint32_t)h[7] << 16);
+  }
+}
+}  // namespace
+
+int conv_tc_pack_device(disn_ctx* c, const float* src, int K, int N, int64_t ld, bool trans, uint8_t* out) {
+  DISN_REQUIRE(K % 64 == 0, "conv_tc_pack_device: K % 64");
+  const int64_t total = (int64_t)((N + 127) / 128) * (K / 64) * 2048;
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, (int64_t)c->num_sms * 16);
+  conv_tc_pack_kernel<<<blocks, 256, 0, c->stream>>>(src, K, N, ld, trans ? 1 : 0, out);
+  c->launches++;
+  DISN_CUDA_OK(cudaGetLastError());
   return 0;
 }
 

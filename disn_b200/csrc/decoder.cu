@@ -17,8 +17,8 @@ struct TapLevels { const float* p[5]; int h[5]; int c[5]; int coff[5]; };
 // out[b,n, coff_l + c] = resampler( tf_resize_bilinear(tap_l -> OHxOW), uv[b,n] )     (model_normalization.py:171-189)
 // one thread = one (point, level, float4 of channels); TF-legacy resize (scale = in/out, no half-pixel) of the four
 // resampler neighbours, then the contrib resampler's four-tap sum (zero outside the map)
-__global__ void point_img_feat_kernel(TapLevels lv, const float* __restrict__ uv, float* __restrict__ out, int B, int64_t N,
-                                      int OH, int OW, int C4total) {
+__global__ void point_img_feat_kernel(TapLevels lv, const float* __restrict__ uv, float* __restrict__ out, int64_t ld, int B,
+                                      int64_t N, int OH, int OW, int C4total) {
   const int64_t total = (int64_t)B * N * C4total;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int c4 = (int)(i % C4total);
@@ -60,7 +60,7 @@ __global__ void point_img_feat_kernel(TapLevels lv, const float* __restrict__ uv
 #undef DISN_RS
       }
     }
-    *reinterpret_cast<float4*>(out + pn * (int64_t)(C4total * 4) + c4 * 4) = acc;
+    *reinterpret_cast<float4*>(out + pn * ld + c4 * 4) = acc;
   }
 }
 
@@ -73,6 +73,29 @@ __global__ void img_points_kernel(const float* __restrict__ pts, const float* __
 }
 
 }  // namespace
+
+// point features of the encoded batch's taps at pts [B,N,3] (device) seen through trans_mat [B,4,3] (device): uv [B,N,2]
+// and out row p = point p's 1472 features, rows ld floats apart (ld % 4 == 0, out 16-byte aligned)
+int gather_point_feat(disn_ctx* c, const float* d_pts, const float* d_tm, int B, int64_t N, float* d_uv, float* out,
+                      int64_t ld) {
+  static const int tapHW[5] = {224, 112, 56, 28, 14};
+  const int64_t n = (int64_t)B * N;
+  const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)c->num_sms * 8);
+  img_points_kernel<<<blocks, 256, 0, c->stream>>>(d_pts, d_tm, d_uv, B, N, c->cfg.clamp_max);
+  TapLevels lv;
+  int off = 0;
+  for (int l = 0; l < 5; ++l) {
+    lv.p[l] = c->taps[l].as<float>(); lv.h[l] = tapHW[l]; lv.c[l] = kTapC[l]; lv.coff[l] = off; off += kTapC[l];
+  }
+  const int64_t total = n * (kLocalFeat / 4);
+  const int blocks2 = (int)std::min<int64_t>((total + 255) / 256, (int64_t)c->num_sms * 16);
+  point_img_feat_kernel<<<blocks2, 256, 0, c->stream>>>(lv, d_uv, out, ld, B, N, c->cfg.img_h, c->cfg.img_w,
+                                                        kLocalFeat / 4);
+  c->launches += 2;
+  DISN_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace disn
 
 using namespace disn;
@@ -84,11 +107,10 @@ extern "C" {
 int disn_point_img_feat(disn_ctx* c, const float* pts, const float* trans_mat, int32_t B, int64_t N, float* out_feat,
                         float* out_uv) {
   DISN_REQUIRE(c && pts && trans_mat && out_feat, "null argument");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_REQUIRE(B == c->enc_B, "batch differs from the encoded batch");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
   if (N <= 0) return 0;
-  static const int tapHW[5] = {224, 112, 56, 28, 14};
   const int64_t n = (int64_t)B * N;
   float *d_pts, *d_uv, *d_feat;
   auto carve = [&](char* base) {
@@ -103,18 +125,7 @@ int disn_point_img_feat(disn_ctx* c, const float* pts, const float* trans_mat, i
   float* tm = c->d_tm.as<float>();
   DISN_CUDA_OK(cudaMemcpyAsync(d_pts, pts, (size_t)n * 3 * 4, cudaMemcpyHostToDevice, c->stream));
   DISN_CUDA_OK(cudaMemcpyAsync(tm, trans_mat, (size_t)B * 12 * 4, cudaMemcpyHostToDevice, c->stream));
-  const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)c->num_sms * 8);
-  img_points_kernel<<<blocks, 256, 0, c->stream>>>(d_pts, tm, d_uv, B, N, c->cfg.clamp_max);
-  TapLevels lv;
-  int off = 0;
-  for (int l = 0; l < 5; ++l) {
-    lv.p[l] = c->taps[l].as<float>(); lv.h[l] = tapHW[l]; lv.c[l] = kTapC[l]; lv.coff[l] = off; off += kTapC[l];
-  }
-  const int64_t total = n * (kLocalFeat / 4);
-  const int blocks2 = (int)std::min<int64_t>((total + 255) / 256, (int64_t)c->num_sms * 16);
-  point_img_feat_kernel<<<blocks2, 256, 0, c->stream>>>(lv, d_uv, d_feat, B, N, c->cfg.img_h, c->cfg.img_w, kLocalFeat / 4);
-  c->launches += 2;
-  DISN_CUDA_OK(cudaGetLastError());
+  if (gather_point_feat(c, d_pts, tm, B, N, d_uv, d_feat, kLocalFeat)) return -1;
   DISN_CUDA_OK(cudaMemcpyAsync(out_feat, d_feat, (size_t)n * kLocalFeat * 4, cudaMemcpyDeviceToHost, c->stream));
   if (out_uv) DISN_CUDA_OK(cudaMemcpyAsync(out_uv, d_uv, (size_t)n * 2 * 4, cudaMemcpyDeviceToHost, c->stream));
   DISN_CUDA_OK(cudaStreamSynchronize(c->stream));
@@ -126,7 +137,7 @@ int disn_point_img_feat(disn_ctx* c, const float* pts, const float* trans_mat, i
 int disn_eval_points_ex(disn_ctx* c, const float* pts, const float* pts_rot, const float* trans_mat, int32_t B, int64_t N,
                         float* out_pred, float* out_uv, float* out_global, float* out_local) {
   DISN_REQUIRE(c && pts && trans_mat && out_pred, "null argument");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_REQUIRE(B == c->enc_B, "batch differs from the encoded batch");
   DISN_CUDA_OK(cudaSetDevice(c->cfg.device));
   if (N <= 0) return 0;

@@ -59,7 +59,7 @@ extern "C" int disn_sdf_metrics(disn_ctx* c, const float* pts, const float* tran
                                 float iso_offset, float sdf_weight, float mask_weight, uint32_t flags, float* pred,
                                 int64_t* count, double* wsum, double* rsum) {
   DISN_REQUIRE(c && pts && trans_mat && gt && count && wsum && rsum, "null argument");
-  DISN_REQUIRE(c->enc_B > 0, "disn_encode has not been called");
+  DISN_REQUIRE(c->enc_B > 0, not_encoded(c));
   DISN_REQUIRE(B == c->enc_B, "batch differs from the encoded batch");
   DISN_REQUIRE(N >= 1, "sdf_metrics: N >= 1 samples per image");
   DISN_REQUIRE(std::isfinite(iso_offset) && std::isfinite(mask_weight) && std::isfinite(sdf_weight) && sdf_weight != 0.f,

@@ -90,6 +90,76 @@ class Engine:
             check(self.lib.disn_load_weight(self._h, name.encode(), a.ctypes.data_as(C.c_void_p), shp, a.ndim))
         check(self.lib.disn_finalize_weights(self._h))
 
+    # -- decoder training ----------------------------------------------------------------------
+    def train_begin(self, beta1: float = 0.5, beta2: float = 0.999, epsilon: float = 1e-8, wd: float = 1e-5,
+                    mask_weight: float = 4.0, sdf_weight: float = 10.0):
+        """Start training the decoder of the loaded weights with TF's Adam (disn_train_begin): zeroed slots,
+        beta powers = betas.  The encoder stays frozen."""
+        cfg = _lib.DisnTrainConfig(beta1, beta2, epsilon, wd, mask_weight, sdf_weight)
+        check(self.lib.disn_train_begin(self._h, C.byref(cfg)))
+        self._train_names = train_var_names()
+
+    def train_step(self, imgs, pts, pts_rot, trans_mat, sdf_gt, lr: float) -> np.ndarray:
+        """One training step (disn_train_step): imgs [B,H,W,3], pts / pts_rot [B,N,3], trans_mat [B,4,3], sdf_gt [B,N] =
+        the fed ground truth (sdf_val - 0.003) -> float64 [5] in TRAIN_LOSS_KEYS order, from the forward pass before the
+        update.  The encoded state is dropped: encode again before inference."""
+        a, p, t, g = _f32(imgs), _f32(pts), _f32(trans_mat), _f32(sdf_gt)
+        if a.ndim != 4 or p.ndim != 3 or p.shape[2] != 3:
+            raise ValueError("imgs must be [B,H,W,C] and pts [B,N,3]")
+        B, N, _ = p.shape
+        pr = None if pts_rot is None else _f32(pts_rot)
+        if a.shape[0] != B or t.size != B * 12 or g.size != B * N or (pr is not None and pr.shape != p.shape):
+            raise ValueError("imgs, pts_rot, trans_mat and sdf_gt must match pts' batch and points")
+        out = np.zeros(5, np.float64)
+        ptr = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)
+        self.batch = 0
+        check(self.lib.disn_train_step(self._h, ptr(a), a.shape[1], a.shape[2], a.shape[3], ptr(p), ptr(pr), ptr(t), ptr(g),
+                                       B, N, float(lr), ptr(out)))
+        return out
+
+    def train_state(self) -> dict:
+        """The training state by TF name: the 24 decoder variables, their `/Adam` and `/Adam_1` slots (TF shapes) and
+        `beta1_power` / `beta2_power` (float32 scalars)."""
+        st = {}
+        for name in self._train_names:
+            n = self._numel(name)
+            for suffix in ("", "/Adam", "/Adam_1"):
+                st[name + suffix] = self.train_get(name + suffix, n).reshape(train_var_shape(name, n))
+        for name in ("beta1_power", "beta2_power"):
+            st[name] = np.float32(self.train_get(name, 1)[0])
+        return st
+
+    def train_phase_ms(self) -> dict:
+        """Device-event milliseconds of the last train_step's phases: encode, gather, forward, loss, backward, adam."""
+        ms = (C.c_float * 6)()
+        check(self.lib.disn_train_phase_ms(self._h, ms))
+        return dict(zip(("encode", "gather", "forward", "loss", "backward", "adam"), list(ms)))
+
+    def train_get(self, name: str, numel: int) -> np.ndarray:
+        """A variable of the context by TF name, flat: a decoder variable or slot, a beta power, or a frozen encoder
+        variable (read only) of numel elements."""
+        out = np.empty(numel, np.float32)
+        check(self.lib.disn_train_get(self._h, name.encode(), out.ctypes.data_as(C.c_void_p), numel))
+        return out
+
+    def _numel(self, name: str) -> int:
+        scope, rest = name.split("/", 1)
+        layer, kind = rest.rsplit("/", 1)
+        cout = _TRAIN_COUT[layer]
+        if kind == "biases":
+            return cout
+        cin = {"fold1/conv1": 3, "fold1/conv2": 64, "fold1/conv3": 256, "fold2/conv2": 512, "fold2/conv5": 256}.get(layer)
+        if cin is None:
+            cin = 512 + (self.cfg.num_classes if scope == "sdfprediction" else 1472)
+        return cin * cout
+
+    def load_train_state(self, state: dict):
+        """Set whatever of train_state()'s names `state` holds (variables, slots, beta powers)."""
+        for name, arr in state.items():
+            a = _f32(arr).reshape(-1)
+            check(self.lib.disn_train_set(self._h, name.encode(), a.ctypes.data_as(C.c_void_p), a.size))
+        self.batch = 0
+
     # -- encoder ------------------------------------------------------------------------------
     def encode(self, imgs):
         a = _f32(imgs)
@@ -701,6 +771,29 @@ class Engine:
         with np.errstate(invalid="ignore", divide="ignore"):
             val = np.where(uni > 0, inter / np.maximum(uni, 1), np.nan)
         return (val, inter, uni, grids) if want_grids else (val, inter, uni)
+
+
+TRAIN_LOSS_KEYS = ("accuracy", "sdf_loss_realvalue", "sdf_loss", "regularization", "overall_loss")
+_TRAIN_COUT = {"fold1/conv1": 64, "fold1/conv2": 256, "fold1/conv3": 512, "fold2/conv1": 512, "fold2/conv2": 256,
+               "fold2/conv5": 1}
+
+
+def train_var_names():
+    """The 24 decoder variables training updates, in the library's order (disn_train_var_name)."""
+    lib = _lib.load()
+    out = []
+    for i in range(24):
+        buf = C.create_string_buffer(128)
+        check(lib.disn_train_var_name(i, buf, len(buf)))
+        out.append(buf.value.decode())
+    return out
+
+
+def train_var_shape(name: str, numel: int):
+    """TF's shape of a decoder variable (or of its Adam slots) with numel elements: [1,1,Cin,Cout] kernels, [Cout] biases."""
+    base = name.split("/Adam")[0]
+    cout = _TRAIN_COUT[base.split("/", 1)[1].rsplit("/", 1)[0]]
+    return (cout,) if base.endswith("/biases") else (1, 1, numel // cout, cout)
 
 
 def batch_losses(count, wsum, rsum, n_values: int):

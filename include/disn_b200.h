@@ -380,6 +380,41 @@ int disn_sdf_metrics(disn_ctx* ctx, const float* pts, const float* trans_mat, co
                      float iso_offset, float sdf_weight, float mask_weight, uint32_t flags, float* pred, int64_t* count,
                      double* wsum, double* rsum);
 
+/* Decoder training with the encoder frozen (train/train_sdf.py with --img_feat_twostream, bn=False; models/
+ * model_normalization.py:169-206,254-299; DESIGN.md 4.12).  The 24 decoder variables (weights and biases of fold1/conv1-3
+ * and fold2/conv1,2,5 in sdfprediction and sdfprediction_imgfeat) of the context are the fp32 masters; TF's Adam updates
+ * them in place.
+ *   disn_train_begin: checks the decoder variables, zeroes the Adam slots, sets beta1_power = beta1, beta2_power = beta2
+ *     and computes the frozen VGG kernels' share of the regularization.  Needs every vgg_16 variable loaded that will
+ *     count (slim.l2_regularizer over its 16 kernels).  Not with tanh_out.
+ *   disn_train_step: one sess.run of the train op on host arrays imgs [B,H,W,3], pts [B,N,3] (`sample_pc`, projected),
+ *     pts_rot [B,N,3] (`sample_pc_rot`, the MLP input; NULL = pts), trans_mat [B,4,3], sdf_gt [B,N] (the fed `sdf`:
+ *     the loader's sdf_val - 0.003), learning rate lr -> losses[5] = accuracy, sdf_loss_realvalue, sdf_loss,
+ *     regularization, overall_loss of the forward pass before the update (float32 values as TF reports them, widened).
+ *     Encodes in groups of 8 images.  Afterwards the encoded state is dropped: every call that needs it fails with an
+ *     error naming the stale state until the next disn_encode, which uses the updated weights.  Synchronous.
+ *   disn_train_get / disn_train_set: by TF name -- a decoder variable, `<var>/Adam`, `<var>/Adam_1`, `beta1_power`,
+ *     `beta2_power` -- n = the element count.  Setting a variable drops the encoded state as a step does.
+ *     Any other loaded variable (the frozen encoder's) can be read, not set.
+ *   disn_train_var_name: the i-th decoder variable's name (i in [0,24)), the order of the diagnostic gradients.
+ *   disn_train_phase_ms: device-event milliseconds of the last step's phases into ms[6]: encode (VGG-16 and the
+ *     embedding copy, all groups), gather (point features), forward, loss (with the regularization norms), backward,
+ *     Adam (0 after the gradient diagnostic). */
+typedef struct disn_train_config {
+  float beta1, beta2, epsilon;   /* AdamOptimizer(lr, beta1=FLAGS.beta1): 0.5, 0.999, 1e-8 */
+  float wd;                      /* weight decay of every kernel (1e-5) */
+  float mask_weight;             /* FLAGS.mask_weight (4) */
+  float sdf_weight;              /* SDF_WEIGHT (10) */
+} disn_train_config;
+void disn_default_train_config(disn_train_config* cfg);
+int disn_train_begin(disn_ctx* ctx, const disn_train_config* cfg);
+int disn_train_step(disn_ctx* ctx, const float* imgs, int32_t H, int32_t W, int32_t C, const float* pts, const float* pts_rot,
+                    const float* trans_mat, const float* sdf_gt, int32_t B, int64_t N, float lr, double* losses);
+int disn_train_get(disn_ctx* ctx, const char* name, float* out, int64_t n);
+int disn_train_set(disn_ctx* ctx, const char* name, const float* data, int64_t n);
+int disn_train_var_name(int32_t i, char* out, int64_t capacity);
+int disn_train_phase_ms(disn_ctx* ctx, float* ms);
+
 /* Kernel launch counter (bench's gpu_launches): number of this library's kernels launched so far. */
 int64_t disn_launch_count(disn_ctx* ctx);
 

@@ -66,6 +66,14 @@ int disn_debug_obj_tokens(const char* text, const int64_t* offsets, const int32_
  * context's encoder products are left as they are. */
 int disn_debug_cam_heads(disn_ctx* ctx, const float* emb, int32_t B, const float* K, float* out_rt, float* out_trans_mat);
 
+/* Diagnostic of decoder training: disn_train_step's gradients of overall_loss without the Adam update -> grads (the 24
+ * variables in disn_train_var_name order, each row-major as TF stores it, wd * W included), pred [B*N], acts (NULL or the
+ * ten layer outputs after ReLU, stream-major, each [B*N][64 | 256 | 512 | 512 | 256]) and losses[5].  Drops the encoded
+ * state as a step does. */
+int disn_debug_train_grads(disn_ctx* ctx, const float* imgs, int32_t H, int32_t W, int32_t C, const float* pts,
+                           const float* pts_rot, const float* trans_mat, const float* sdf_gt, int32_t B, int64_t N,
+                           float* grads, float* pred, float* acts, double* losses);
+
 #ifdef __cplusplus
 }
 #endif
