@@ -21,11 +21,12 @@
 //   * weights are pre-split and pre-swizzled on the host into the exact shared-memory images of the B operand
 //     (32 KB per 128 output features x 64 k), packed in consumption order and streamed by the bulk-copy engine
 //     (cp.async.bulk) through a 3-slot mbarrier ring.  Half-stages alternate between the two warpgroups, so each
-//     (slot, warpgroup) has its own "landed" and "empty" barrier and every barrier phase has one waiter.  A warpgroup
-//     issues all MMAs of a half-stage as one commit group and waits for it once; each of its warps then arrives on the
-//     slot's empty barrier, and its first thread refills the slot with half-stage g + 3 when all four have (no
-//     separate producer warp: the register file is allocated to warps in groups of four, and the consumers need all
-//     of it);
+//     (slot, warpgroup) has its own "landed" and "empty" barrier and every barrier phase has one waiter.  A consumer
+//     warpgroup issues all MMAs of a half-stage as one commit group and waits for it once; each of its warps then
+//     arrives on the slot's empty barrier.  A third, producer warpgroup refills the ring: one of its threads waits for
+//     each slot's release and issues the next half-stage's bulk copy, in half-stage order, so the refill is off the
+//     consumers' path from one MMA group to the next.  The register file is split with setmaxnreg: the producer
+//     warpgroup gives back all but 24 registers per thread and the consumers rise to 240 (launched at 168);
 //   * the small per-stream parameters (biases, fold1/conv1, fold2/conv5) are read from global memory through the
 //     read-only cache: the lanes of a warp read different features, and the constant bank would serialise them.
 #include <algorithm>
@@ -45,7 +46,12 @@ namespace disn {
 namespace {
 
 constexpr int PTS = 64;               // points per tile (the wgmma M)
-constexpr int NCONS = 256;            // two consumer warpgroups
+constexpr int NCONS = 256;            // two consumer warpgroups: threads [0, 256)
+constexpr int NTHREADS = NCONS + 128; // and the producer warpgroup: threads [256, 384)
+// registers per thread after the roles split (setmaxnreg); launched at 65536 / 384 rounded down to 8, i.e. 168
+constexpr int REG_PRODUCER = 24;
+constexpr int REG_CONSUMER = 240;
+static_assert(128 * REG_PRODUCER + NCONS * REG_CONSUMER <= 65536, "register split exceeds the register file");
 constexpr int NSLOT = 3;              // weight ring slots
 constexpr int W_TILE = 16384;         // 128 rows x 64 k x 2 B (SW128)
 constexpr int W8_TILE = 8192;         // 128 rows x 64 k x 1 B (SW64)
@@ -140,7 +146,7 @@ __device__ __forceinline__ void store_pair(uint8_t* x, uint32_t o16, uint32_t o8
 
 // the consumers hold two 64-register accumulators (plus the 64-register correction accumulator of MODE_F16F8)
 template <int kMode>
-__global__ void __launch_bounds__(NCONS, 1)
+__global__ void __launch_bounds__(NTHREADS, 1)
 point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
                  int64_t tiles_per_img) {
   extern __shared__ uint8_t smem_raw[];
@@ -164,17 +170,29 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
     tc::fence_barrier_init();
   }
   __syncthreads();
-  const uint32_t total_hs = (uint32_t)my_tiles * HS_PER_TILE;
-  // half-stage g -> slot g % NSLOT, consumed by warpgroup g & 1
-  auto load_stage = [&](uint32_t g) {
-    const uint32_t slot = g % NSLOT;
-    tc::mbar_arrive_expect_tx(&full[slot][g & 1], HS_BYTES);
-    tc::bulk_g2s(s.w[slot], wpk + (size_t)(g % HS_PER_TILE) * HS_BYTES, HS_BYTES, &full[slot][g & 1]);
-  };
-  if (tid == 0)
-    for (uint32_t g = 0; g < NSLOT && g < total_hs; ++g) load_stage(g);
 
-  // ===================== consumers =====================
+  // ===================== producer =====================
+  if (tid >= NCONS) {
+    tc::setmaxnreg_dec<REG_PRODUCER>();
+    if (tid == NCONS) {
+      // half-stage g -> slot g % NSLOT, consumed by warpgroup g & 1.  It reuses the slot of half-stage q = g - NSLOT,
+      // which warpgroup q & 1 releases on empty[q % NSLOT][q & 1]: that (slot, warpgroup) pair's use number q / 6.
+      const uint32_t total_hs = (uint32_t)my_tiles * HS_PER_TILE;
+      for (uint32_t g = 0; g < total_hs; ++g) {
+        const uint32_t slot = g % NSLOT;
+        if (g >= NSLOT) {
+          const uint32_t q = g - NSLOT;
+          tc::mbar_wait_inline(&empty[slot][q & 1], (q / (2 * NSLOT)) & 1u);
+        }
+        tc::mbar_arrive_expect_tx(&full[slot][g & 1], HS_BYTES);
+        tc::bulk_g2s(s.w[slot], wpk + (size_t)(g % HS_PER_TILE) * HS_BYTES, HS_BYTES, &full[slot][g & 1]);
+      }
+    }
+    return;
+  }
+
+  // ===================== consumers (threads [0, NCONS): tid is the consumer thread index) =====================
+  tc::setmaxnreg_inc<REG_CONSUMER>();
   const int h = warp >> 2;                       // warpgroup: output features [128h, 128h + 128) of each N block
   const int wi = warp & 3;
   const int r0 = wi * 16 + (lane >> 2);          // accumulator rows r0, r0 + 8
@@ -282,20 +300,14 @@ point_tc_kernel(PointJob job, const uint8_t* __restrict__ wpk,
             tc::wgmma_commit();
             tc::wgmma_wait<0>();
             tc::acc_fence(acc[nb]);
-            // this warp is done with the slot; the warpgroup's first thread refills it once all four warps are.  The
-            // other warps arrive without waiting on anything, so that wait always completes.
-            const bool refill = g + NSLOT < total_hs;
-            if (refill && lane == 0) tc::mbar_arrive(&empty[slot][h]);
+            // this warp is done with the slot; the producer refills it once all four warps are
+            if (lane == 0) tc::mbar_arrive(&empty[slot][h]);
             if constexpr (kMode == MODE_F16F8) {
               if (k1 || k2) {
                 tc::acc_fence(tmp);
 #pragma unroll
                 for (int i = 0; i < 64; ++i) acc[nb][i] += tmp[i];
               }
-            }
-            if (refill && (tid & 127) == 0) {
-              tc::mbar_wait(&empty[slot][h], par);
-              load_stage(g + NSLOT);
             }
             g += 2;
           }
@@ -429,7 +441,7 @@ int launch_var(disn_ctx* c, const PointJob& job, const void* wpk, int grid, int 
     DISN_CUDA_OK(cudaFuncSetAttribute(point_tc_kernel<kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     c->attr_done.insert(key);
   }
-  point_tc_kernel<kMode><<<grid, NCONS, smem, c->stream>>>(job, reinterpret_cast<const uint8_t*>(wpk), tiles_per_img);
+  point_tc_kernel<kMode><<<grid, NTHREADS, smem, c->stream>>>(job, reinterpret_cast<const uint8_t*>(wpk), tiles_per_img);
   return 0;
 }
 

@@ -1,5 +1,5 @@
-// sm_90a building blocks for the tensor-core kernels: mbarrier, cluster, bulk copy (TMA engine), GMMA shared-memory
-// descriptors and warpgroup MMA (wgmma.mma_async, m64n128) wrappers (inline PTX).
+// sm_90a building blocks for the tensor-core kernels: mbarrier, cluster, register reallocation (setmaxnreg), bulk copy
+// (TMA engine), GMMA shared-memory descriptors and warpgroup MMA (wgmma.mma_async, m64n128) wrappers (inline PTX).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -64,7 +64,9 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
 // Bounded wait: a protocol bug traps (reported as a launch failure) instead of hanging the GPU.
 // The timer is consulted only every 4096 failed polls: reading %globaltimer costs hundreds of cycles and
 // must stay off the common path (try_wait itself suspends the thread until the phase flips or a HW time slice).
-static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity) {
+// mbar_wait_inline is the whole wait without a call, for a warpgroup that has lowered its register limit
+// (setmaxnreg.dec): ptxas fails to allocate a kernel whose reduced-register code calls mbar_wait_slow.
+__device__ __forceinline__ void mbar_wait_inline(uint64_t* bar, uint32_t parity) {
   uint64_t t0 = 0;
   for (uint32_t spins = 1;; ++spins) {
     if (mbar_try_wait(bar, parity)) return;
@@ -75,9 +77,25 @@ static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parit
     }
   }
 }
+static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity) { mbar_wait_inline(bar, parity); }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   mbar_wait_slow(bar, parity);
+}
+
+// ---------------------------------------------------------------- register reallocation ---------------
+// Change the calling warpgroup's per-thread register limit to N (24..256, a multiple of 8).  Every warp of the
+// warpgroup must execute the same instruction.  `dec` returns registers to the CTA's pool; `inc` blocks until the pool
+// can grant them, so a kernel that splits roles decreases in one warpgroup what it increases in the others.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  static_assert(N >= 24 && N <= 256 && N % 8 == 0, "setmaxnreg: 24..256 in steps of 8");
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  static_assert(N >= 24 && N <= 256 && N % 8 == 0, "setmaxnreg: 24..256 in steps of 8");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 
 // ---------------------------------------------------------------- proxies / fences -------------------

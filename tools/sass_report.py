@@ -5,6 +5,12 @@ Compiles disn_b200/csrc/point_tc.cu with the library's nvcc flags into a tempora
 operand-mode instantiation of point_tc_kernel: registers, spill stores and loads, whether ptxas serialised the warpgroup
 MMAs (warning C7512), and instruction counts per segment of the kernel body, cut at every BAR.SYNC.
 
+The kernel launches three warpgroups and splits the register file with setmaxnreg.  ptxas reports the launch count;
+the report adds each role's budget from the SASS (USETMAXREG.TRY_ALLOC for the consumers, USETMAXREG.DEALLOC for the
+producer) and the highest register each role's code uses, which shows whether the consumers really use more than the
+launch count.  The producer's code (from its USETMAXREG.DEALLOC to its EXIT) is counted as its own segment and left
+out of the consumer segments.
+
 Every epilogue loop is fully unrolled, so a segment's static counts are the instructions each thread runs per tile
 there; an MMA segment holds a `#pragma unroll 1` loop over K slices and its counts are per loop body.  Segments are
 named from the kernel's structure: a segment with warpgroup MMAs is a layer's MMA loop, the segment after it that
@@ -37,6 +43,7 @@ MODES = {"0": "bf16x3", "1": "f16f8"}
 INT_OPS = {"LOP3", "IADD3", "IMAD", "LEA", "SHF", "VIADD", "MOV"}
 COLUMNS = ("total", "int", "LDG", "STS", "F2FP", "GMMA", "LDL/STL")
 _INSN = re.compile(r"^\s*/\*[0-9a-f]+\*/\s+(?:@!?U?P[T0-9]+\s+)?([A-Z0-9_.]+)")
+_REG = re.compile(r"\bR(\d+)\b")
 
 
 def compile_kernel(src: str, tmp: str):
@@ -80,7 +87,7 @@ def ptxas_info(log: str):
 
 
 def kernels(sass: str):
-    """kernel mode -> list of opcodes in program order"""
+    """kernel mode -> list of (opcode, instruction text) in program order"""
     out, cur = {}, None
     for line in sass.splitlines():
         m = re.search(r"Function : \w*point_tc_kernelILi(\d)E", line)
@@ -92,8 +99,25 @@ def kernels(sass: str):
             continue
         m = _INSN.match(line)
         if m and cur is not None:
-            cur.append(m.group(1))
+            cur.append((m.group(1), line.split(";")[0]))
     return out
+
+
+def max_reg(insns):
+    """highest general register Rn the instructions name (-1 if none)"""
+    return max((int(r) for _, text in insns for r in _REG.findall(text)), default=-1)
+
+
+def split_roles(insns):
+    """-> (consumer and common instructions, producer instructions, consumer budget, producer budget).  The producer
+    region runs from USETMAXREG.DEALLOC to the next EXIT; budgets are None when the kernel has no setmaxnreg."""
+    alloc = next((i for i, (op, _) in enumerate(insns) if op.startswith("USETMAXREG.TRY_ALLOC")), None)
+    dealloc = next((i for i, (op, _) in enumerate(insns) if op.startswith("USETMAXREG.DEALLOC")), None)
+    budget = lambda i: int(re.search(r"(0x[0-9a-f]+|\d+)\s*$", insns[i][1]).group(1), 0) if i is not None else None
+    if dealloc is None:
+        return insns, [], budget(alloc), None
+    end = next((i for i in range(dealloc, len(insns)) if insns[i][0] == "EXIT"), len(insns) - 1)
+    return insns[:dealloc] + insns[end + 1:], insns[dealloc:end + 1], budget(alloc), budget(dealloc)
 
 
 def count(ops):
@@ -157,12 +181,24 @@ def main():
         regs, st, ld, c7512 = info.get(mode, [None, None, None, False])
         print("\n== point_tc_kernel, %s: %s registers, %s B spill stores, %s B spill loads, C7512 %s"
               % (mode, regs, st, ld, "PRESENT (MMAs serialised)" if c7512 else "absent"))
-        segs = segments(ks.get(mode, []))
+        insns = ks.get(mode, [])
+        rest, prod, b_cons, b_prod = split_roles(insns)
+        if b_cons is None and b_prod is None:
+            print("   one register budget: %s at launch (no setmaxnreg); highest register used R%d"
+                  % (regs, max_reg(insns)))
+        else:
+            alloc = next(i for i, (op, _) in enumerate(rest) if op.startswith("USETMAXREG.TRY_ALLOC"))
+            print("   register budgets: %s at launch; consumers setmaxnreg %s, highest register used R%d; "
+                  "producer setmaxnreg %s, highest register used R%d"
+                  % (regs, b_cons, max_reg(rest[alloc:]), b_prod, max_reg(prod)))
+        segs = segments([op for op, _ in rest])
         names = name_segments(segs, mode)
         print("%-30s" % "segment" + "".join("%9s" % c for c in COLUMNS))
         epi = dict.fromkeys(COLUMNS, 0)
         mma = dict.fromkeys(COLUMNS, 0)
         body = count([op for s in segs for op in s])
+        if prod:
+            print("%-30s" % "   producer" + "".join("%9d" % v for v in count([op for op, _ in prod]).values()))
         spill_in = []
         for i, s in enumerate(segs):
             c = count(s)
