@@ -60,12 +60,20 @@ def forward(W, emb, feat, pts_rot, masks=None, absolute=False):
     return pred, cache
 
 
+def weight_mask(gt, mask_weight=MASK_WEIGHT):
+    """get_loss's weight_mask: mask_weight where gt <= 0.01, else 1.  TF compares the float32 ground truth with the
+    float32 constant 0.01, so that is what is written here.  It equals the float64 comparison g <= 0.01 for float32 g:
+    float32(0.01) lies below 0.01 and is the largest float32 not above it, so no float32 falls between the two."""
+    g32 = np.asarray(gt, np.float32).reshape(-1)
+    return np.where(g32 <= np.float32(0.01), np.float64(mask_weight), 1.0)
+
+
 def loss_terms(pred, gt, signs=None, weights=None, sdf_weight=SDF_WEIGHT, mask_weight=MASK_WEIGHT):
     """get_loss's sdf terms in float64: (sdf_loss, sdf_loss_realvalue, accuracy, dpred).  gt = the fed ground truth."""
     p = np.asarray(pred, np.float64).reshape(-1)
     g = np.asarray(gt, np.float64).reshape(-1)
     d = g * sdf_weight - p
-    w = np.where(g <= 0.01, mask_weight, 1.0) if weights is None else np.asarray(weights, np.float64).reshape(-1)
+    w = weight_mask(gt, mask_weight) if weights is None else np.asarray(weights, np.float64).reshape(-1)
     sg = np.sign(d) if signs is None else np.asarray(signs, np.float64).reshape(-1)
     P = p.size
     sdf_loss = 1000.0 * np.sum(np.abs(d) * w) / P
@@ -97,15 +105,16 @@ def backward(W, cache, dpred, wd=WD, absolute=False):
     return grads
 
 
-def step_grads(W, emb, feat, pts, pts_rot, gt, masks=None, signs=None, weights=None, absolute=False, wd=WD):
+def step_grads(W, emb, feat, pts, pts_rot, gt, masks=None, signs=None, weights=None, absolute=False, wd=WD,
+               sdf_weight=SDF_WEIGHT, mask_weight=MASK_WEIGHT):
     """One step's (pred, grads) in float64; absolute=True gives the magnitude sums of the same passes."""
     pred, cache = forward(W, emb, feat, pts_rot, masks=masks, absolute=absolute)
     if absolute:
         g = np.asarray(gt, np.float64).reshape(-1)
-        w = np.where(g <= 0.01, MASK_WEIGHT, 1.0) if weights is None else np.asarray(weights, np.float64).reshape(-1)
+        w = weight_mask(gt, mask_weight) if weights is None else np.asarray(weights, np.float64).reshape(-1)
         dpred = 1000.0 / g.size * w
     else:
-        dpred = loss_terms(pred, gt, signs, weights)[3]
+        dpred = loss_terms(pred, gt, signs, weights, sdf_weight, mask_weight)[3]
     return pred, backward(W, cache, dpred, wd=wd, absolute=absolute)
 
 
@@ -120,10 +129,10 @@ def regularization(weights, wd=WD):
     return total
 
 
-def reported_losses(pred, gt, weights, wd=WD):
+def reported_losses(pred, gt, weights, wd=WD, sdf_weight=SDF_WEIGHT, mask_weight=MASK_WEIGHT):
     """The five values train_sdf.py reports for a step, rounded to float32 as TF reports them: accuracy,
     sdf_loss_realvalue, sdf_loss, regularization, overall_loss."""
-    sdf_loss, real, acc, _ = loss_terms(pred, gt)
+    sdf_loss, real, acc, _ = loss_terms(pred, gt, sdf_weight=sdf_weight, mask_weight=mask_weight)
     reg = regularization(weights, wd)
     loss32 = np.float32(sdf_loss)
     return np.array([np.float32(acc), np.float32(real), loss32, np.float32(reg), np.float32(loss32 + np.float32(reg))],
